@@ -20,7 +20,7 @@ SYMBOLS = [
     "ifb200_batch_create", "ifb200_batch_enqueue", "ifb200_batch_color_matrix", "ifb200_batch_sync",
     "ifb200_batch_destroy", "ifb200_batch_set_option", "ifb200_batch_kernel_launches", "ifb200_batch_host_profile",
     "ifb200_batch_fused_jobs", "ifb200_batch_generic_jobs", "ifb200_batch_tile_jobs", "ifb200_batch_ring_status", "ifb200_hv_plan_tables",
-    "ifb200_block_scale_u8", "ifb200_batch_block_scale",
+    "ifb200_block_scale_u8", "ifb200_batch_block_scale", "ifb200_round_corners_bgra8", "ifb200_batch_round_corners",
 ]
 
 
@@ -33,6 +33,14 @@ class ResampleDesc(C.Structure):
         ("filter", C.c_int32), ("sharpen_percent", C.c_float), ("linear", C.c_int32),
         ("alpha_meaningful", C.c_int32), ("compose", C.c_int32), ("matte_bgra", C.c_uint8 * 4),
         ("color_matrix", C.c_void_p),
+    ]
+
+
+class RoundCornersDesc(C.Structure):
+    """struct ifb200_round_corners_desc"""
+    _fields_ = [
+        ("px", C.c_void_p), ("w", C.c_uint32), ("h", C.c_uint32), ("stride", C.c_uint32),
+        ("mode", C.c_int32), ("radius", C.c_float * 4), ("matte_bgra", C.c_uint8 * 4),
     ]
 
 
@@ -118,6 +126,10 @@ def lib() -> C.CDLL:
     L.ifb200_block_scale_u8.restype = C.c_int
     L.ifb200_batch_block_scale.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int, C.c_int, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_block_scale.restype = C.c_int
+    L.ifb200_round_corners_bgra8.argtypes = [C.POINTER(RoundCornersDesc), C.c_char_p, C.c_size_t]
+    L.ifb200_round_corners_bgra8.restype = C.c_int
+    L.ifb200_batch_round_corners.argtypes = [C.c_void_p, C.POINTER(RoundCornersDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
+    L.ifb200_batch_round_corners.restype = C.c_int
     L.ifb200_batch_ring_status.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_ring_status.restype = C.c_int
     _lib = L

@@ -1170,6 +1170,71 @@ void detect_content_locked(ifb200_batch* b, const uint8_t* px, uint32_t w, uint3
     if (!ifb::detect_content_from_codes(codes, w, h, rect, nullptr)) IFB_THROW(IFB200_ERR_INVALID_STATE, "whitespace walk failed");
 }
 
+// flow_bitmap_bgra_clear_around_rounded_corners (graphics/rounded_corners.rs:187-346).  Argument checks of one job; degenerate radii
+// are not errors (the planner gives them the reference's meaning).
+void round_corners_validate(const ifb200_round_corners_desc& d) {
+    if (d.mode < IFB200_CORNERS_PERCENTAGE || d.mode > IFB200_CORNERS_PIXELS_CUSTOM) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "unknown corners mode %d", d.mode);
+    if (d.w == 0 || d.h == 0) return;
+    if (!d.px) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null bitmap pointer");
+    if (d.stride < d.w * 4ull || (d.stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "stride smaller than a BGRA row or not a multiple of 4");
+    if ((uint64_t)d.w * d.h > 0xffffffffull) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "bitmap too large");
+}
+// the planned job of a validated, non-empty descriptor, on bitmap (px, stride)
+ifb::RcJob round_corners_job(const ifb200_round_corners_desc& d, uint8_t* px, uint32_t stride) {
+    ifb::RcJob job{};
+    if (!ifb::round_corners_plan(d.mode, d.radius, d.w, d.h, &job)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "unknown corners mode %d", d.mode);
+    job.px = px; job.stride = stride;
+    job.matte = (uint32_t)d.matte_bgra[0] | ((uint32_t)d.matte_bgra[1] << 8) | ((uint32_t)d.matte_bgra[2] << 16) | ((uint32_t)d.matte_bgra[3] << 24);
+    return job;
+}
+// Jobs and their cover rectangles cut into CTA tiles of at most kRcTilePixels pixels
+struct RcWork {
+    std::vector<ifb::RcJob> jobs; std::vector<ifb::RcTile> tiles;
+    void add(const ifb::RcJob& job, const std::vector<ifb::RcRect>& rects) {
+        const uint32_t j = (uint32_t)jobs.size();
+        jobs.push_back(job);
+        for (const auto& r : rects) {
+            const uint64_t area = (uint64_t)r.w * r.h;
+            for (uint64_t f = 0; f < area; f += ifb::kRcTilePixels)
+                tiles.push_back({j, r.x0, r.y0, r.w, (uint32_t)f, (uint32_t)std::min<uint64_t>(ifb::kRcTilePixels, area - f)});
+        }
+    }
+};
+// ONE launch for every tile of `wk`, asynchronous on `st` (none when no job touches a pixel)
+void round_corners_launch(ifb200_batch* b, const RcWork& wk, cudaStream_t st) {
+    if (wk.tiles.empty()) return;
+    if (wk.tiles.size() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
+    DeviceScope dev_scope_(b->device);
+    const size_t jb = (wk.jobs.size() * sizeof(ifb::RcJob) + 255) / 256 * 256, tb = wk.tiles.size() * sizeof(ifb::RcTile);
+    cudaEvent_t ev;
+    uint8_t* hbuf = static_cast<uint8_t*>(b->stage(jb + tb, &ev));
+    memcpy(hbuf, wk.jobs.data(), wk.jobs.size() * sizeof(ifb::RcJob));
+    memcpy(hbuf + jb, wk.tiles.data(), tb);
+    uint8_t* dbuf = nullptr;
+    CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&dbuf), jb + tb, st));
+    AsyncFree dbuf_guard{dbuf, st};
+    CUDA_OK(cudaMemcpyAsync(dbuf, hbuf, jb + tb, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaEventRecord(ev, st));
+    round_corners_kernel<<<(unsigned)wk.tiles.size(), ifb::kRcThreads, 0, st>>>(reinterpret_cast<const ifb::RcJob*>(dbuf),
+                                                                              reinterpret_cast<const ifb::RcTile*>(dbuf + jb), b->tables);
+    CUDA_OK(cudaGetLastError());
+    b->launches++;
+}
+void round_corners_locked(ifb200_batch* b, const ifb200_round_corners_desc* d, size_t n, cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    for (size_t i = 0; i < n; ++i) round_corners_validate(d[i]);           // all-or-nothing, before any device use
+    RcWork wk;
+    std::vector<ifb::RcRect> rects;
+    for (size_t i = 0; i < n; ++i) {
+        if (d[i].w == 0 || d[i].h == 0) continue;
+        const ifb::RcJob job = round_corners_job(d[i], d[i].px, d[i].stride);
+        rects.clear();
+        ifb::round_corners_cover(job, rects);
+        wk.add(job, rects);
+    }
+    round_corners_launch(b, wk, st);
+}
+
 // Pageable host bitmaps (imageflow's Bitmap buffers are plain Vecs, aligned_buffer.rs:40-43): cudaMemcpy2DAsync from pageable memory
 // is staged by the driver on the calling thread (about 10 GB/s, and it does not overlap).  The drop-in path therefore stages such
 // bitmaps itself: the rows are copied into a pinned buffer of the pipeline slot by a few host threads in parallel, the pinned buffer
@@ -1541,6 +1606,14 @@ int ifb200_batch_block_scale(ifb200_batch* b, const uint8_t* dev_in, uint32_t in
     });
 }
 
+int ifb200_batch_round_corners(ifb200_batch* b, const ifb200_round_corners_desc* d, size_t n, void* stream, char* err, size_t cap) {
+    return guarded(err, cap, [&] {
+        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
+        std::lock_guard<std::mutex> lk(b->mu);
+        round_corners_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
+    });
+}
+
 int ifb200_batch_sync(ifb200_batch* b, char* err, size_t cap) {
     return guarded(err, cap, [&] {
         if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
@@ -1700,6 +1773,37 @@ int ifb200_apply_matte_bgra8(uint8_t* px, uint32_t w, uint32_t h, uint32_t strid
         CUDA_OK(cudaMemcpy2DAsync(sl.d_cv, pitch, px, stride, (size_t)w * 4, h, cudaMemcpyHostToDevice, st));
         apply_matte_locked(b, sl.d_cv, w, h, (uint32_t)pitch, matte_bgra, st);
         CUDA_OK(cudaMemcpy2DAsync(px, stride, sl.d_cv, pitch, (size_t)w * 4, h, cudaMemcpyDeviceToHost, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+    });
+}
+
+// Only the planned cover travels: each rectangle is one 2D copy into the same place of a device image laid out like the frame, the
+// kernel runs on that image, each rectangle comes back with one 2D copy.  Rectangles that are only filled are not uploaded.
+int ifb200_round_corners_bgra8(const ifb200_round_corners_desc* d, char* err, size_t cap) {
+    return guarded(err, cap, [&] {
+        if (!d) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor");
+        round_corners_validate(*d);
+        if (d->w == 0 || d->h == 0) return;
+        HostCtx& c = host_ctx();
+        ifb200_batch* b = c.batch;
+        std::lock_guard<std::mutex> lk(b->mu);
+        DeviceScope dev_scope_(b->device);
+        HostSlot& sl = c.slot[0];
+        cudaStream_t st = sl.stream;
+        const size_t pitch = ((size_t)d->w * 4 + 63) / 64 * 64;
+        ensure(sl.d_cv, sl.cap_cv, pitch * d->h, st);
+        const ifb::RcJob job = round_corners_job(*d, sl.d_cv, (uint32_t)pitch);
+        std::vector<ifb::RcRect> rects;
+        ifb::round_corners_cover(job, rects);
+        auto dev_at = [&](const ifb::RcRect& r) { return sl.d_cv + (size_t)r.y0 * pitch + (size_t)r.x0 * 4; };
+        auto host_at = [&](const ifb::RcRect& r) { return d->px + (size_t)r.y0 * d->stride + (size_t)r.x0 * 4; };
+        for (const auto& r : rects)
+            if (!r.fill_only) CUDA_OK(cudaMemcpy2DAsync(dev_at(r), pitch, host_at(r), d->stride, (size_t)r.w * 4, r.h, cudaMemcpyHostToDevice, st));
+        RcWork wk;
+        wk.add(job, rects);
+        round_corners_launch(b, wk, st);
+        for (const auto& r : rects)
+            CUDA_OK(cudaMemcpy2DAsync(host_at(r), d->stride, dev_at(r), pitch, (size_t)r.w * 4, r.h, cudaMemcpyDeviceToHost, st));
         CUDA_OK(cudaStreamSynchronize(st));
     });
 }

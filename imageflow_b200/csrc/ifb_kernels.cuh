@@ -18,18 +18,15 @@
 
 #include <type_traits>
 
+#include "ifb_round_corners.h"     // RcJob / RcTile: planned on the host, read by round_corners_kernel
+
 namespace ifbk {
 
 // ---------------------------------------------------------------- device-side descriptors (their own file: tests/cpu_emu includes it too)
 #include "ifb_types.cuh"
 
 // ---------------------------------------------------------------- scalar helpers
-// lut.rs:4-8
-__device__ __forceinline__ uint32_t lut_encode(const uint8_t* __restrict__ lut16k, float lin) {
-    float s = __fmul_rn(lin, 16383.0f);
-    s = fminf(fmaxf(s, 0.0f), 16383.0f);     // NaN -> 0, as `NaN as usize`
-    return (uint32_t)__ldg(lut16k + (int)s);
-}
+#include "ifb_lut.cuh"
 __device__ __forceinline__ uint32_t encode(bool linear, const uint8_t* __restrict__ lut16k, float v) {
     return linear ? lut_encode(lut16k, v) : uchar_clamp_ff(__fmul_rn(255.0f, v));   // color.rs:59-69
 }
@@ -351,6 +348,9 @@ __global__ void __launch_bounds__(256) apply_byte_maps_bgra8_kernel(uint8_t* __r
 // ---------------------------------------------------------------- whitespace detection (SURVEY.md section 8(f), item 4, second half)
 // In its own file so that tests/ can also execute this very source under a CPU emulation of the CUDA built-ins it uses.
 #include "ifb_whitespace_kernel.cuh"
+
+// ---------------------------------------------------------------- rounded corners (SURVEY.md section 8(f), item 5); own file for tests/cpu_emu
+#include "ifb_round_corners_kernel.cuh"
 
 // ---------------------------------------------------------------- decode-time JPEG block scalers (SURVEY.md section 8(f), item 1)
 #include "ifb_idct_kernel.cuh"

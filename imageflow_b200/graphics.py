@@ -9,7 +9,7 @@ from typing import Optional, Sequence
 
 import numpy as np
 
-from ._lib import ResampleDesc, lib
+from ._lib import ResampleDesc, RoundCornersDesc, lib
 
 
 class Filter(enum.IntEnum):
@@ -194,6 +194,52 @@ def white_balance_srgb_mut(bitmap: BitmapWindow, threshold: Optional[float] = No
     _check(lib().ifb200_white_balance_srgb_bgra8(bitmap.ptr, bitmap.w, bitmap.h, bitmap.stride, -1.0 if threshold is None else float(threshold), buf, 512), buf)
 
 
+@dataclass(frozen=True)
+class RoundCornersMode:
+    """imageflow_types RoundCornersMode (lib.rs:1257-1268).  `kind` is the enum's declaration index (ifb200_corners_mode);
+    `radius` is (top_left, top_right, bottom_right, bottom_left), the field order of the *Custom variants."""
+    kind: int
+    radius: tuple = (0.0, 0.0, 0.0, 0.0)
+    PERCENTAGE, PIXELS, CIRCLE, PERCENTAGE_CUSTOM, PIXELS_CUSTOM = range(5)
+
+    @classmethod
+    def percentage(cls, p: float) -> "RoundCornersMode":
+        return cls(cls.PERCENTAGE, (float(p), 0.0, 0.0, 0.0))
+
+    @classmethod
+    def pixels(cls, p: float) -> "RoundCornersMode":
+        return cls(cls.PIXELS, (float(p), 0.0, 0.0, 0.0))
+
+    @classmethod
+    def circle(cls) -> "RoundCornersMode":
+        return cls(cls.CIRCLE)
+
+    @classmethod
+    def percentage_custom(cls, top_left: float, top_right: float, bottom_right: float, bottom_left: float) -> "RoundCornersMode":
+        return cls(cls.PERCENTAGE_CUSTOM, (float(top_left), float(top_right), float(bottom_right), float(bottom_left)))
+
+    @classmethod
+    def pixels_custom(cls, top_left: float, top_right: float, bottom_right: float, bottom_left: float) -> "RoundCornersMode":
+        return cls(cls.PIXELS_CUSTOM, (float(top_left), float(top_right), float(bottom_right), float(bottom_left)))
+
+
+def _fill_corners_desc(d: RoundCornersDesc, window: BitmapWindow, mode: RoundCornersMode, matte_bgra) -> None:
+    if window.pixel_layout != "BGRA":                                          # rounded_corners.rs:192-194
+        raise FlowError(ErrorKind.InvalidArgument, "Only BGRA supported for rounded corners")
+    d.px = window.ptr; d.w = window.w; d.h = window.h; d.stride = window.stride
+    d.mode = int(mode.kind)
+    d.radius = (C.c_float * 4)(*mode.radius)
+    d.matte_bgra = (C.c_uint8 * 4)(*matte_bgra)
+
+
+def flow_bitmap_bgra_clear_around_rounded_corners(window: BitmapWindow, mode: RoundCornersMode, matte_bgra) -> None:
+    """graphics/rounded_corners.rs:187-346, in place on a HOST window; matte_bgra = background_color as BGRA8."""
+    d = RoundCornersDesc()
+    _fill_corners_desc(d, window, mode, matte_bgra)
+    buf = C.create_string_buffer(512)
+    _check(lib().ifb200_round_corners_bgra8(C.byref(d), buf, 512), buf)
+
+
 def flow_scale_spatial(samples: np.ndarray, n: int, srgb: bool = False) -> np.ndarray:
     """flow_scale_spatial[_srgb]_{n}x{n} (c_components/lib/codecs_jpeg_idct_fast.c) applied to every 8x8 block of a plane of
     samples (H x W uint8, both multiples of 8; host memory): returns the (H/8*n) x (W/8*n) plane."""
@@ -369,6 +415,17 @@ class Batch:
         buf = C.create_string_buffer(512)
         _check(lib().ifb200_batch_whitespace_codes(self._h, bitmap.ptr, bitmap.w, bitmap.h, bitmap.stride, int(bool(bitmap.alpha_meaningful)),
                                                    int(threshold), dev_codes_ptr, self._stream(stream), buf, 512), buf)
+
+    def round_corners(self, jobs, stream=None) -> None:
+        """graphics/rounded_corners.rs:187-346 on DEVICE windows, in place, all jobs in one kernel launch (asynchronous on
+        `stream`).  jobs: iterable of (BitmapWindow, RoundCornersMode, matte_bgra); no two windows may share a pixel."""
+        jobs = list(jobs)
+        arr = (RoundCornersDesc * len(jobs))()
+        for d, (window, mode, matte) in zip(arr, jobs):
+            _fill_corners_desc(d, window, mode, matte)
+        self._keep.append([j[0]._keep for j in jobs])
+        buf = C.create_string_buffer(512)
+        _check(lib().ifb200_batch_round_corners(self._h, arr, len(jobs), self._stream(stream), buf, 512), buf)
 
     def flip_vertical(self, bitmap: BitmapWindow, stream=None) -> None:
         """graphics/flip.rs:10-22 on a DEVICE bitmap, in place."""

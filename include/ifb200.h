@@ -160,6 +160,24 @@ int ifb200_white_balance_srgb_bgra8(uint8_t* px, uint32_t w, uint32_t h, uint32_
 int ifb200_block_scale_u8(const uint8_t* in, uint32_t in_stride, uint32_t blocks_x, uint32_t blocks_y, uint8_t* out, uint32_t out_stride,
                           int n, int srgb, char* err, size_t err_cap);
 
+/* Replaces flow_bitmap_bgra_clear_around_rounded_corners (graphics/rounded_corners.rs:187-346), the op behind RoundImageCorners /
+ * s.roundcorners= (flow/nodes/round_corners.rs:62-84): pixels outside the rounded corners become the matte, the arcs are
+ * anti-aliased over it in linear light, in place.  [SURVEY.md section 8(f), item 5]
+ * Modes: imageflow_types RoundCornersMode (lib.rs:1257-1268), in declaration order.  Radii that the reference clamps, ceils or
+ * truncates (negative, NaN, infinite, oversized) behave exactly as they do there; they are not errors. */
+enum ifb200_corners_mode { IFB200_CORNERS_PERCENTAGE = 0, IFB200_CORNERS_PIXELS = 1, IFB200_CORNERS_CIRCLE = 2,
+                           IFB200_CORNERS_PERCENTAGE_CUSTOM = 3, IFB200_CORNERS_PIXELS_CUSTOM = 4 };
+typedef struct ifb200_round_corners_desc {
+    uint8_t* px; uint32_t w, h, stride;   /* BGRA8 window, in place; stride in bytes */
+    int32_t  mode;                        /* enum ifb200_corners_mode */
+    float    radius[4];                   /* top_left, top_right, bottom_right, bottom_left (the field order of
+                                             RoundCornersMode::*Custom); [0] alone for PERCENTAGE / PIXELS; unused for CIRCLE */
+    uint8_t  matte_bgra[4];               /* background_color.to_color_32().to_bgra8() */
+} ifb200_round_corners_desc;
+/* HOST window, synchronous.  Only the pixels the op can touch travel to the GPU and back (a few rectangles at the corners; rectangles
+ * that are only filled with the matte are not uploaded). */
+int ifb200_round_corners_bgra8(const ifb200_round_corners_desc* d, char* err, size_t err_cap);
+
 /* ---- device-resident batch API (the metric path; not in the reference) -----------------------
  * descs[i].in / .canvas are DEVICE pointers on the batch's device; color_matrix stays a HOST pointer.
  * enqueue is asynchronous on `cuda_stream`, a cudaStream_t with the usual CUDA meaning (NULL = the legacy
@@ -197,6 +215,10 @@ int  ifb200_batch_detect_content(ifb200_batch* b, const uint8_t* dev_px, uint32_
  * Asynchronous on `cuda_stream`; ifb200_detect_content_from_codes() walks a host copy of it. */
 int  ifb200_batch_whitespace_codes(ifb200_batch* b, const uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, int alpha_meaningful,
                                    uint32_t threshold, uint8_t* dev_codes, void* cuda_stream, char* err, size_t err_cap);
+/* Rounded corners of n DEVICE windows (d[i].px on the batch's device) in ONE kernel launch, asynchronous on `cuda_stream`.  The jobs
+ * of one call must not overlap in memory (no two windows may share a pixel): they run concurrently.  Argument errors are reported
+ * before anything is enqueued. */
+int  ifb200_batch_round_corners(ifb200_batch* b, const ifb200_round_corners_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
 int  ifb200_batch_sync(ifb200_batch* b, char* err, size_t err_cap);
 void ifb200_batch_destroy(ifb200_batch* b);
 /* knobs / introspection (benchmarks, tests) */

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Measurement of the SURVEY.md section 8(f) neighbours of the resample path that are built: transpose, flips, white balance and detect_content
+"""Measurement of the SURVEY.md section 8(f) neighbours of the resample path that are built: transpose, flips, white balance, detect_content
+and rounded corners
 (the reference benchmarks transposes at 4K / 8K in benches/bench_graphics.rs:9-62).  Inputs resident in HBM, CUDA events on
 the launching stream, >= 3 warm-up calls; a set of 64 different images per size (>= 2 GB, far larger than L2) is cycled so that
 no call finds its data in cache.  One JSON line per (operation, size) with the HBM roofline of the kernel: algorithmic
@@ -113,8 +114,65 @@ def main():
                           "whole_call_ms": call_ms, "host_walk_ms": walk_ms, "host_walk_pixels_visited": visited,
                           "cpu_oracle_ms_1_thread": cpu_ms, "rect": list(rect), "bit_exact_vs_oracle": bool(tuple(rect) == tuple(want) == tuple(rect_w)),
                           "images_cycled": n}))
+        if w == 3840:
+            round_corners_rows(batch, imgs, host, stream, pk, src)
         del imgs, outs, codes
         torch.cuda.empty_cache()
+
+
+def round_corners_rows(batch, imgs, host, stream, pk, src):
+    """graphics/rounded_corners.rs on 4K frames: the op touches a few rectangles per frame, so per image it is far below a launch's
+    cost; the rows compare one batch call over 64 images (one launch) with 64 one-image calls, time the drop-in call (only the
+    planned rectangles travel) by wall clock against the oracle's loop on one host thread, and check the result bit for bit.
+    Algorithmic bytes: 4 written per pixel filled with the matte, 4 read + 4 written per blended pixel (the oracle's touch mask)."""
+    from tests import round_corners_oracle as rco
+    rco.lib()                                          # compiled on first use: not part of the oracle's time
+    n, h, w = imgs.shape[0], imgs.shape[1], imgs.shape[2]
+    matte = (20, 40, 60, 255)
+    for label, mode in (("pixels_100", ifb.RoundCornersMode.pixels(100)), ("circle", ifb.RoundCornersMode.circle())):
+        wins = [ifb.BitmapWindow.from_torch(imgs[i]) for i in range(n)]
+        one_call = lambda: batch.round_corners([(wn, mode, matte) for wn in wins], stream)
+        per_image = lambda: [batch.round_corners([(wn, mode, matte)], stream) for wn in wins]
+        times = {}
+        for name, fn in (("batch_64_one_call", one_call), ("64_one_image_calls", per_image)):
+            for _ in range(3):
+                fn()
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            reps = 10
+            e0.record()
+            for _ in range(reps):
+                fn()
+            e1.record(); torch.cuda.synchronize()
+            times[name] = e0.elapsed_time(e1) / reps
+        exp = host.copy()
+        t0 = time.perf_counter()
+        mask = rco.round_corners(exp, mode.kind, mode.radius, matte, want_mask=True)
+        cpu_ms = (time.perf_counter() - t0) * 1e3
+        filled, blended = int((mask == 1).sum()), int((mask == 2).sum())
+        alg = 4 * filled + 8 * blended
+        d = torch.from_numpy(host).to(imgs.device)
+        batch.round_corners([(ifb.BitmapWindow.from_torch(d), mode, matte)], stream)
+        torch.cuda.synchronize()
+        ok_batch = bool(np.array_equal(d.cpu().numpy(), exp))
+        hw = host.copy()
+        win = ifb.BitmapWindow.from_numpy(hw)
+        ifb.flow_bitmap_bgra_clear_around_rounded_corners(win, mode, matte)
+        ok_drop = bool(np.array_equal(hw, exp))
+        drop = []
+        for _ in range(5):
+            hw[...] = host
+            t0 = time.perf_counter()
+            ifb.flow_bitmap_bgra_clear_around_rounded_corners(win, mode, matte)
+            drop.append((time.perf_counter() - t0) * 1e3)
+        ms = times["batch_64_one_call"] / n
+        print(json.dumps({"op": "round_corners", "mode": label, "size": f"{w}x{h}", "pixels_filled": filled, "pixels_blended": blended,
+                          "batch_64_one_call_ms": times["batch_64_one_call"], "64_one_image_calls_ms": times["64_one_image_calls"],
+                          "ms_per_image_in_batch": ms, "mpx_touched_per_s": (filled + blended) / ms / 1e3,
+                          "roofline": {"bound": "hbm", "achieved": alg / ms / 1e6, "peak": pk, "unit": "GB/s", "frac": alg / ms / 1e6 / pk,
+                                       "peak_source": src, "algorithmic_bytes_per_image": alg},
+                          "drop_in_wall_ms_median": float(np.median(drop)), "cpu_oracle_ms_1_thread": cpu_ms,
+                          "bit_exact_vs_oracle": ok_batch and ok_drop, "images_per_batch": n}))
 
 
 if __name__ == "__main__":
