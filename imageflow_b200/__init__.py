@@ -10,6 +10,8 @@ Host-side mirror of the reference seam (paths relative to the imageflow checkout
   flow/nodes/white_balance.rs   white_balance_srgb_mut (histogram.rs, area thresholds, byte maps)
   graphics/whitespace.rs:284    detect_content (code map on the GPU, the reference's window walk on the host)
   graphics/rounded_corners.rs:187  flow_bitmap_bgra_clear_around_rounded_corners, RoundCornersMode (imageflow_types)
+  graphics/bitmaps.rs:1504,1570, graphics/copy_rect.rs:12  fill_rectangle, normalize_unused_alpha, copy_rectangle (Batch.canvas:
+      FillRect, EnableTransparency, CopyRectToCanvas, ExpandCanvas; WatermarkRedDot, Region, RegionPercent as helpers)
   c_components/lib/codecs_jpeg_idct_fast.c  flow_scale_spatial[_srgb]_NxN (decode-time JPEG block scalers)
 All arithmetic runs in hand-written sm_90a kernels inside libifb200.so (include/ifb200.h);
 this package only marshals arguments.  Nothing here imports the CPU oracle.
@@ -18,7 +20,8 @@ from .graphics import (Batch, apply_matte, BitmapCompositing, BitmapWindow, Erro
                        WorkingFloatspace, color_filter_matrix, device_count, plan_probe, populate_weights, scale_and_render, scale_and_render_many,
                        window_bgra32_apply_color_matrix, bitmap_window_transpose, flow_bitmap_bgra_flip_vertical_safe,
                        flow_bitmap_bgra_flip_horizontal_safe, white_balance_srgb_mut, detect_content, detect_content_from_codes, flow_scale_spatial,
-                       RoundCornersMode, flow_bitmap_bgra_clear_around_rounded_corners)
+                       RoundCornersMode, flow_bitmap_bgra_clear_around_rounded_corners,
+                       FillRect, CopyRectToCanvas, ExpandCanvas, EnableTransparency, new_canvas, watermark_red_dot, region, region_percent)
 from ._lib import LIB_PATH, ResampleDesc, lib
 
 __all__ = [
@@ -26,5 +29,6 @@ __all__ = [
     "WorkingFloatspace", "color_filter_matrix", "device_count", "plan_probe", "populate_weights", "scale_and_render", "scale_and_render_many",
     "window_bgra32_apply_color_matrix", "bitmap_window_transpose", "flow_bitmap_bgra_flip_vertical_safe",
     "flow_bitmap_bgra_flip_horizontal_safe", "white_balance_srgb_mut", "detect_content", "detect_content_from_codes", "flow_scale_spatial",
-    "RoundCornersMode", "flow_bitmap_bgra_clear_around_rounded_corners", "LIB_PATH", "ResampleDesc", "lib",
+    "RoundCornersMode", "flow_bitmap_bgra_clear_around_rounded_corners",
+    "FillRect", "CopyRectToCanvas", "ExpandCanvas", "EnableTransparency", "new_canvas", "watermark_red_dot", "region", "region_percent", "LIB_PATH", "ResampleDesc", "lib",
 ]

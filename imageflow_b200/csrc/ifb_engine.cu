@@ -1200,21 +1200,32 @@ struct RcWork {
         }
     }
 };
-// ONE launch for every tile of `wk`, asynchronous on `st` (none when no job touches a pixel)
-void round_corners_launch(ifb200_batch* b, const RcWork& wk, cudaStream_t st) {
-    if (wk.tiles.empty()) return;
-    if (wk.tiles.size() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
-    DeviceScope dev_scope_(b->device);
-    const size_t jb = (wk.jobs.size() * sizeof(ifb::RcJob) + 255) / 256 * 256, tb = wk.tiles.size() * sizeof(ifb::RcTile);
+// The job and tile lists of one flat launch in one stream-ordered device allocation on `st` (staged through pinned memory): returns
+// it, with the jobs at offset 0 and the tiles at *tiles_at.  The caller launches, then frees it on `st`.
+template <class J, class T>
+uint8_t* upload_work(ifb200_batch* b, const std::vector<J>& jobs, const std::vector<T>& tiles, cudaStream_t st, size_t* tiles_at) {
+    if (tiles.size() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
+    const size_t jb = (jobs.size() * sizeof(J) + 255) / 256 * 256, tb = tiles.size() * sizeof(T);
     cudaEvent_t ev;
     uint8_t* hbuf = static_cast<uint8_t*>(b->stage(jb + tb, &ev));
-    memcpy(hbuf, wk.jobs.data(), wk.jobs.size() * sizeof(ifb::RcJob));
-    memcpy(hbuf + jb, wk.tiles.data(), tb);
+    memcpy(hbuf, jobs.data(), jobs.size() * sizeof(J));
+    memcpy(hbuf + jb, tiles.data(), tb);
     uint8_t* dbuf = nullptr;
     CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&dbuf), jb + tb, st));
     AsyncFree dbuf_guard{dbuf, st};
     CUDA_OK(cudaMemcpyAsync(dbuf, hbuf, jb + tb, cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaEventRecord(ev, st));
+    dbuf_guard.release();
+    *tiles_at = jb;
+    return dbuf;
+}
+// ONE launch for every tile of `wk`, asynchronous on `st` (none when no job touches a pixel)
+void round_corners_launch(ifb200_batch* b, const RcWork& wk, cudaStream_t st) {
+    if (wk.tiles.empty()) return;
+    DeviceScope dev_scope_(b->device);
+    size_t jb = 0;
+    uint8_t* dbuf = upload_work(b, wk.jobs, wk.tiles, st, &jb);
+    AsyncFree dbuf_guard{dbuf, st};
     round_corners_kernel<<<(unsigned)wk.tiles.size(), ifb::kRcThreads, 0, st>>>(reinterpret_cast<const ifb::RcJob*>(dbuf),
                                                                               reinterpret_cast<const ifb::RcTile*>(dbuf + jb), b->tables);
     CUDA_OK(cudaGetLastError());
@@ -1233,6 +1244,27 @@ void round_corners_locked(ifb200_batch* b, const ifb200_round_corners_desc* d, s
         wk.add(job, rects);
     }
     round_corners_launch(b, wk, st);
+}
+
+// The canvas operations of ifb200_batch_canvas (ifb_canvas.h): every descriptor is checked before anything is planned or enqueued,
+// then all jobs run in ONE launch (none when no job writes a pixel).
+void canvas_locked(ifb200_batch* b, const ifb200_canvas_desc* d, size_t n, cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    for (size_t i = 0; i < n; ++i) {
+        const std::string why = ifb::canvas_check(d[i]);
+        if (!why.empty()) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "canvas job %zu: %s", i, why.c_str());
+    }
+    ifb::CvWork wk;
+    for (size_t i = 0; i < n; ++i) ifb::canvas_plan(d[i], wk);
+    if (wk.tiles.empty()) return;
+    DeviceScope dev_scope_(b->device);
+    size_t tb = 0;
+    uint8_t* dbuf = upload_work(b, wk.items, wk.tiles, st, &tb);
+    AsyncFree dbuf_guard{dbuf, st};
+    canvas_kernel<<<(unsigned)wk.tiles.size(), ifb::kCvThreads, 0, st>>>(reinterpret_cast<const ifb::CvItem*>(dbuf),
+                                                                       reinterpret_cast<const ifb::CvTile*>(dbuf + tb));
+    CUDA_OK(cudaGetLastError());
+    b->launches++;
 }
 
 // Pageable host bitmaps (imageflow's Bitmap buffers are plain Vecs, aligned_buffer.rs:40-43): cudaMemcpy2DAsync from pageable memory
@@ -1611,6 +1643,14 @@ int ifb200_batch_round_corners(ifb200_batch* b, const ifb200_round_corners_desc*
         if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
         std::lock_guard<std::mutex> lk(b->mu);
         round_corners_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
+    });
+}
+
+int ifb200_batch_canvas(ifb200_batch* b, const ifb200_canvas_desc* d, size_t n, void* stream, char* err, size_t cap) {
+    return guarded(err, cap, [&] {
+        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
+        std::lock_guard<std::mutex> lk(b->mu);
+        canvas_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
     });
 }
 

@@ -19,6 +19,7 @@
 #include <type_traits>
 
 #include "ifb_round_corners.h"     // RcJob / RcTile: planned on the host, read by round_corners_kernel
+#include "ifb_canvas.h"            // CvItem / CvTile: planned on the host, read by canvas_kernel
 
 namespace ifbk {
 
@@ -351,6 +352,9 @@ __global__ void __launch_bounds__(256) apply_byte_maps_bgra8_kernel(uint8_t* __r
 
 // ---------------------------------------------------------------- rounded corners (SURVEY.md section 8(f), item 5); own file for tests/cpu_emu
 #include "ifb_round_corners_kernel.cuh"
+
+// ---------------------------------------------------------------- canvas operations (fill, copy, expand, normalise alpha); own file for tests/cpu_emu
+#include "ifb_canvas_kernel.cuh"
 
 // ---------------------------------------------------------------- decode-time JPEG block scalers (SURVEY.md section 8(f), item 1)
 #include "ifb_idct_kernel.cuh"

@@ -9,7 +9,7 @@ from typing import Optional, Sequence
 
 import numpy as np
 
-from ._lib import ResampleDesc, RoundCornersDesc, lib
+from ._lib import CanvasDesc, ResampleDesc, RoundCornersDesc, lib
 
 
 class Filter(enum.IntEnum):
@@ -240,6 +240,176 @@ def flow_bitmap_bgra_clear_around_rounded_corners(window: BitmapWindow, mode: Ro
     _check(lib().ifb200_round_corners_bgra8(C.byref(d), buf, 512), buf)
 
 
+# ---------------------------------------------------------------- canvas operations (Batch.canvas), named after the imageflow_types nodes
+@dataclass
+class FillRect:
+    """Node::FillRect { x1, y1, x2, y2, color } on `window` (bitmaps.rs:1504-1562); color = Color::to_bgra8() bytes (b, g, r, a)."""
+    window: BitmapWindow
+    x1: int
+    y1: int
+    x2: int
+    y2: int
+    color: Sequence[int]
+
+
+@dataclass
+class CopyRectToCanvas:
+    """Node::CopyRectToCanvas { from_x, from_y, w, h, x, y }: copy_rectangle(input, canvas, ...) (graphics/copy_rect.rs:12-97)."""
+    input: BitmapWindow
+    canvas: BitmapWindow
+    from_x: int
+    from_y: int
+    w: int
+    h: int
+    x: int
+    y: int
+
+
+@dataclass
+class ExpandCanvas:
+    """Node::ExpandCanvas { left, top, right, bottom, color } of `input` (clone_crop_fill_expand.rs:224-260).  The new canvas is
+    allocated by Batch.canvas (a uint8 CUDA tensor, rows padded to 64 bytes as bitmaps.rs:803-804) unless `canvas` is given."""
+    input: BitmapWindow
+    left: int
+    top: int
+    right: int
+    bottom: int
+    color: Sequence[int]
+    canvas: Optional[BitmapWindow] = None
+
+
+@dataclass
+class EnableTransparency:
+    """EnableTransparencyMutDef (flow/nodes/enable_transparency.rs:70-86): a Bgr32 window gets A = 255 and becomes Bgra32."""
+    window: BitmapWindow
+
+
+def _device_of(w: BitmapWindow, default: int) -> int:
+    k = w._keep
+    return k.device.index if getattr(getattr(k, "device", None), "type", None) == "cuda" else default
+
+
+def new_canvas(w: int, h: int, device: int = 0, alpha_meaningful: bool = True) -> BitmapWindow:
+    """Bitmap::create_u8's buffer on the GPU (bitmaps.rs:803-804): an uninitialised w x h BGRA8 window of a uint8 CUDA tensor whose
+    rows are padded to 64 bytes."""
+    import torch
+    stride = (w * 4 + 63) // 64 * 64
+    t = torch.empty((h, stride // 4, 4), dtype=torch.uint8, device=torch.device("cuda", device))[:, :w]
+    return BitmapWindow(t.data_ptr(), w, h, stride, alpha_meaningful, _keep=t)
+
+
+def watermark_red_dot(window: BitmapWindow) -> list:
+    """flow/nodes/watermark_red_dot.rs:26-39: a 3x3 FillRect of FF0000 in the bottom-right corner of frames larger than 3x3."""
+    if window.w > 3 and window.h > 3:
+        return [FillRect(window, window.w - 3, window.h - 3, window.w, window.h, (0, 0, 255, 255))]
+    return []
+
+
+def region(window: BitmapWindow, x1: int, y1: int, x2: int, y2: int, color, device: int = 0):
+    """RegionDef::expand (clone_crop_fill_expand.rs:390-451): the op that makes Region { x1, y1, x2, y2, background_color } of
+    `window` -- an ExpandCanvas of the cropped window, or, when the region misses the window, a FillRect of a new canvas of the
+    window's format (CreateCanvas)."""
+    if y2 <= y1 or x2 <= x1:
+        raise FlowError(ErrorKind.InvalidArgument, f"Invalid coordinates: {x1},{y1} {x2},{y2} should describe the top-left and "
+                                                   "bottom-right corners of the region in pixels. Not a rectangle.")
+    if x1 >= window.w or y1 >= window.h or x2 <= 0 or y2 <= 0:
+        cv = new_canvas(x2 - x1, y2 - y1, _device_of(window, device), window.alpha_meaningful)
+        return FillRect(cv, 0, 0, cv.w, cv.h, tuple(color))
+    crop = window.window(min(window.w, max(0, x1)), min(window.h, max(0, y1)), min(window.w, max(0, x2)), min(window.h, max(0, y2)))
+    return ExpandCanvas(crop, max(0, -x1), max(0, -y1), max(0, x2 - window.w), max(0, y2 - window.h), tuple(color))
+
+
+def _round_f32(v) -> int:
+    """`(f32).round() as i32`: half away from zero, saturating, NaN -> 0"""
+    import math
+    v = float(v)
+    if v != v:
+        return 0
+    r = math.copysign(math.floor(abs(v) + 0.5), v) if math.isfinite(v) else v
+    return int(max(-2 ** 31, min(2 ** 31 - 1, r)))
+
+
+def region_percent(window: BitmapWindow, left: float, top: float, right: float, bottom: float, color, device: int = 0):
+    """RegionPercentDef (clone_crop_fill_expand.rs:265-350): get_coords in f32, then region()."""
+    if bottom <= top or right <= left:
+        raise FlowError(ErrorKind.InvalidArgument, f"Invalid coordinates: {left},{top} {right},{bottom} should describe the top-left and "
+                                                   "bottom-right corners of the region in percentages. Not a rectangle.")
+    f, hundred = np.float32, np.float32(100)
+    x1 = _round_f32(f(window.w) * f(left) / hundred)
+    y1 = _round_f32(f(window.h) * f(top) / hundred)
+    x2 = _round_f32(f(window.w) * f(right) / hundred)
+    y2 = _round_f32(f(window.h) * f(bottom) / hundred)
+    if x2 < x1:
+        x2 = x1 + 1
+    if y2 < y1:
+        y2 = y1 + 1
+    return region(window, x1, y1, x2, y2, color, device)
+
+
+_FILL_RECT, _COPY_RECT, _EXPAND, _NORMALIZE_ALPHA = range(4)          # enum ifb200_canvas_op
+
+
+def _fill_canvas_desc(d: CanvasDesc, op, device: int):
+    """Fills d for one op; returns the window the op writes (its metadata updated as the reference updates the bitmap's)."""
+    def target(w: BitmapWindow):
+        d.px = w.ptr; d.w = w.w; d.h = w.h; d.stride = w.stride; d.alpha_meaningful = int(bool(w.alpha_meaningful))
+
+    def source(w: BitmapWindow):
+        d.in_ = w.ptr; d.in_w = w.w; d.in_h = w.h; d.in_stride = w.stride; d.in_alpha_meaningful = int(bool(w.alpha_meaningful))
+
+    wins = [getattr(op, n) for n in ("window", "input", "canvas") if getattr(op, n, None) is not None]
+    if any(w.pixel_layout != "BGRA" for w in wins):
+        raise FlowError(ErrorKind.InvalidArgument, "Only BGRA supported for canvas operations")
+    if isinstance(op, FillRect):
+        w = op.window
+        if w.compose == BitmapCompositing.BlendWithMatte and (op.x1, op.y1, op.x2, op.y2) != (0, 0, w.w, w.h):   # bitmaps.rs:1512-1519
+            raise FlowError(ErrorKind.InvalidArgument, "Cannot draw a rectangle on a sub-rectangle of a bitmap in BlendWithMatte mode")
+        d.op = _FILL_RECT
+        target(w)
+        d.x1, d.y1, d.x2, d.y2 = op.x1, op.y1, op.x2, op.y2
+        d.color_bgra = (C.c_uint8 * 4)(*op.color)
+        return lambda: w
+    if isinstance(op, CopyRectToCanvas):
+        d.op = _COPY_RECT
+        target(op.canvas); source(op.input)
+        d.x1, d.y1, d.x2, d.y2, d.cw, d.ch = op.from_x, op.from_y, op.x, op.y, op.w, op.h
+
+        def done(cv=op.canvas, inp=op.input):                     # copy_rect.rs:37, :47-54
+            cv.compose = BitmapCompositing.BlendWithSelf
+            if inp.alpha_meaningful:
+                cv.alpha_meaningful = True
+            return cv
+        return done
+    if isinstance(op, ExpandCanvas):
+        d.op = _EXPAND
+        inp = op.input
+        w, h = inp.w + op.left + op.right, inp.h + op.top + op.bottom
+        am = bool(inp.alpha_meaningful) if op.color[3] == 255 else True      # clone_crop_fill_expand.rs:239
+        cv = op.canvas if op.canvas is not None else new_canvas(w, h, device)
+        target(cv); source(inp)
+        d.x1, d.y1, d.x2, d.y2 = op.left, op.top, op.right, op.bottom
+        d.color_bgra = (C.c_uint8 * 4)(*op.color)
+
+        def done():
+            cv.alpha_meaningful = am
+            cv.compose = BitmapCompositing.BlendWithSelf
+            return cv
+        return done
+    if isinstance(op, EnableTransparency):
+        w = op.window
+        if w.alpha_meaningful:                                   # enable_transparency.rs:74-78
+            raise FlowError(ErrorKind.InvalidArgument, "Need Bgr32 input image to convert to bgra32")
+        d.op = _NORMALIZE_ALPHA
+        target(w)
+
+        def done():
+            w.alpha_meaningful = True
+            w.compose = BitmapCompositing.BlendWithSelf
+            return w
+        return done
+    raise FlowError(ErrorKind.InvalidArgument, f"not a canvas operation: {op!r}")
+
+
 def flow_scale_spatial(samples: np.ndarray, n: int, srgb: bool = False) -> np.ndarray:
     """flow_scale_spatial[_srgb]_{n}x{n} (c_components/lib/codecs_jpeg_idct_fast.c) applied to every 8x8 block of a plane of
     samples (H x W uint8, both multiples of 8; host memory): returns the (H/8*n) x (W/8*n) plane."""
@@ -426,6 +596,20 @@ class Batch:
         self._keep.append([j[0]._keep for j in jobs])
         buf = C.create_string_buffer(512)
         _check(lib().ifb200_batch_round_corners(self._h, arr, len(jobs), self._stream(stream), buf, 512), buf)
+
+    def canvas(self, ops, stream=None) -> list:
+        """Canvas operations on DEVICE windows, all in one kernel launch (none when no op writes a pixel), asynchronous on `stream`.
+        ops: FillRect, CopyRectToCanvas, ExpandCanvas, EnableTransparency.  No op may write what another op of the call reads or
+        writes.  Returns, per op, the window it wrote (ExpandCanvas: the new canvas), with alpha_meaningful and compose updated as
+        the reference updates the bitmap; nothing is changed when an argument is rejected."""
+        ops = list(ops)
+        arr = (CanvasDesc * len(ops))()
+        done = [_fill_canvas_desc(d, op, self.device) for d, op in zip(arr, ops)]
+        buf = C.create_string_buffer(512)
+        _check(lib().ifb200_batch_canvas(self._h, arr, len(ops), self._stream(stream), buf, 512), buf)
+        out = [f() for f in done]
+        self._keep.append([[getattr(op, n, None) for n in ("window", "input", "canvas")] for op in ops] + [w._keep for w in out])
+        return out
 
     def flip_vertical(self, bitmap: BitmapWindow, stream=None) -> None:
         """graphics/flip.rs:10-22 on a DEVICE bitmap, in place."""

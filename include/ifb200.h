@@ -178,6 +178,31 @@ typedef struct ifb200_round_corners_desc {
  * that are only filled with the matte are not uploaded). */
 int ifb200_round_corners_bgra8(const ifb200_round_corners_desc* d, char* err, size_t err_cap);
 
+/* The canvas layer of a flow graph, on BGRA8 windows (alpha_meaningful = 1 is the reference's Bgra32, 0 its Bgr32):
+ *   FILL_RECT        BitmapWindowMut::fill_rectangle(color, x1, y1, x2, y2) (graphics/bitmaps.rs:1504-1562): FillRect, WatermarkRedDot.
+ *                    x2 == x1 or y2 == y1 is a no-op (even out of bounds); otherwise the rectangle must lie inside the window.
+ *   COPY_RECT        copy_rectangle(in, canvas, x1, y1, x2, y2, cw, ch) (graphics/copy_rect.rs:12-97): CopyRectToCanvas.  A Bgr32
+ *                    canvas under a Bgra32 input first gets A = 255 over its whole window; a Bgr32 input under a Bgra32 canvas gets
+ *                    A = 255 over its whole window, in place.  Then the rows are copied as raw bytes (stride padding is not).
+ *   EXPAND           ExpandCanvas { left = x1, top = y1, right = x2, bottom = y2, color } (flow/nodes/clone_crop_fill_expand.rs:224-260)
+ *                    into the caller's new canvas px (w = in_w + left + right, h = in_h + top + bottom): the border becomes color,
+ *                    the interior the input, as COPY_RECT into a Bgr32 (color opaque, a == 255, and input Bgr32) or Bgra32 canvas.
+ *                    The descriptor's alpha_meaningful is not read: that format rule decides it.
+ *   NORMALIZE_ALPHA  normalize_unused_alpha (graphics/bitmaps.rs:1564-1576): A = 255 over the window unless alpha_meaningful.
+ * Each pixel is written once (EXPAND fills only the border).  Bitmap metadata checks (BGRA only, BlendWithMatte sub-rectangles,
+ * EnableTransparency on a Bgra32 bitmap) stay with the caller.  24-bit inputs are not supported. */
+enum ifb200_canvas_op { IFB200_CANVAS_FILL_RECT = 0, IFB200_CANVAS_COPY_RECT = 1, IFB200_CANVAS_EXPAND = 2, IFB200_CANVAS_NORMALIZE_ALPHA = 3 };
+typedef struct ifb200_canvas_desc {
+    int32_t  op;                                               /* enum ifb200_canvas_op */
+    uint8_t* px; uint32_t w, h, stride; int32_t alpha_meaningful;             /* the window written: FILL / NORMALIZE target, COPY
+                                                                                 canvas, EXPAND's new canvas; stride in bytes   */
+    uint8_t* in; uint32_t in_w, in_h, in_stride; int32_t in_alpha_meaningful; /* COPY / EXPAND source; not const: a Bgr32 input
+                                                                                 under a Bgra32 canvas gets A = 255 in place     */
+    uint32_t x1, y1, x2, y2;   /* FILL: x, y, x2, y2.  COPY: from_x, from_y, to_x, to_y.  EXPAND: left, top, right, bottom */
+    uint32_t cw, ch;           /* COPY: w, h */
+    uint8_t  color_bgra[4];    /* FILL / EXPAND: Color::to_bgra8() */
+} ifb200_canvas_desc;
+
 /* ---- device-resident batch API (the metric path; not in the reference) -----------------------
  * descs[i].in / .canvas are DEVICE pointers on the batch's device; color_matrix stays a HOST pointer.
  * enqueue is asynchronous on `cuda_stream`, a cudaStream_t with the usual CUDA meaning (NULL = the legacy
@@ -219,6 +244,11 @@ int  ifb200_batch_whitespace_codes(ifb200_batch* b, const uint8_t* dev_px, uint3
  * of one call must not overlap in memory (no two windows may share a pixel): they run concurrently.  Argument errors are reported
  * before anything is enqueued. */
 int  ifb200_batch_round_corners(ifb200_batch* b, const ifb200_round_corners_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
+/* Canvas operations (ifb200_canvas_desc) on n DEVICE windows in ONE kernel launch, none when no job writes a pixel; asynchronous on
+ * `cuda_stream`.  No job may write what another job of the same call reads or writes; a job's input and canvas windows must not
+ * overlap in memory.  Argument errors are reported before anything is enqueued.  There is no host-buffer variant: on a host bitmap
+ * these ops are a memset / memcpy, cheaper than a trip to the GPU. */
+int  ifb200_batch_canvas(ifb200_batch* b, const ifb200_canvas_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
 int  ifb200_batch_sync(ifb200_batch* b, char* err, size_t err_cap);
 void ifb200_batch_destroy(ifb200_batch* b);
 /* knobs / introspection (benchmarks, tests) */

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Measurement of the SURVEY.md section 8(f) neighbours of the resample path that are built: transpose, flips, white balance, detect_content
-and rounded corners
+and rounded corners; `bench_neighbours.py canvas` measures the canvas operations alone (canvas_rows)
 (the reference benchmarks transposes at 4K / 8K in benches/bench_graphics.rs:9-62).  Inputs resident in HBM, CUDA events on
 the launching stream, >= 3 warm-up calls; a set of 64 different images per size (>= 2 GB, far larger than L2) is cycled so that
 no call finds its data in cache.  One JSON line per (operation, size) with the HBM roofline of the kernel: algorithmic
@@ -175,5 +175,113 @@ def round_corners_rows(batch, imgs, host, stream, pk, src):
                           "bit_exact_vs_oracle": ok_batch and ok_drop, "images_per_batch": n}))
 
 
+def _card():
+    """the card's name and power limit, read in the same run as the numbers"""
+    import subprocess
+    try:
+        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True,
+                            timeout=30).stdout.strip()
+    except Exception:
+        pl = "unknown"
+    return {"gpu": torch.cuda.get_device_name(0), "power_limit": pl}
+
+
+def _time_ms(fn, reps=10):
+    for _ in range(3):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        fn()
+    e1.record(); torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / reps
+
+
+def _copy_ceiling_ms(alg_bytes):
+    """a torch device-to-device copy that moves alg_bytes in all (alg_bytes / 2 read, alg_bytes / 2 written)"""
+    n = max(alg_bytes // 2, 1)
+    a = torch.empty(n, dtype=torch.uint8, device="cuda"); b = torch.empty_like(a)
+    ms = _time_ms(lambda: b.copy_(a))
+    del a, b
+    return ms
+
+
+def canvas_rows():
+    """Canvas operations (Batch.canvas) on frames resident in HBM.  Algorithmic bytes: 4 written per canvas pixel plus 4 read per
+    copied pixel.  Each row also times a torch device-to-device copy of the same number of bytes as a practical ceiling."""
+    card = _card()
+    pk, src = peak()
+    b = ifb.Batch(0)
+    stream = torch.cuda.current_stream().cuda_stream
+
+    def row(name, ms, alg, **kw):
+        cm = _copy_ceiling_ms(alg)
+        print(json.dumps({"op": "canvas", "row": name, "ms": ms, "algorithmic_bytes": alg, "achieved_gbs": alg / ms / 1e6,
+                          "frac_of_peak": alg / ms / 1e6 / pk, "peak_gbs": pk, "peak_source": src, "torch_copy_same_bytes_ms": cm,
+                          "frac_of_torch_copy": cm / ms, **kw, **card}))
+
+    # ExpandCanvas: 64 x 3840x2160 -> 3840x2880, opaque colour, one call
+    n, w, h, H = 64, 3840, 2160, 2880
+    ins = (torch.randn((n, h, w, 4), device="cuda") * 40 + 128).clamp_(0, 255).to(torch.uint8)
+    outs = torch.empty((n, H, w, 4), dtype=torch.uint8, device="cuda")
+    iw = [ifb.BitmapWindow.from_torch(ins[i]) for i in range(n)]
+    ow = [ifb.BitmapWindow.from_torch(outs[i]) for i in range(n)]
+    top = (H - h) // 2
+    ops = [ifb.ExpandCanvas(iw[i], 0, top, 0, H - h - top, (10, 20, 30, 255), canvas=ow[i]) for i in range(n)]
+    ms = _time_ms(lambda: b.canvas(ops, stream))
+    want = torch.full((H - h - top, w, 4), 0, dtype=torch.uint8, device="cuda"); want[...] = torch.tensor((10, 20, 30, 255), dtype=torch.uint8)
+    ok = bool(torch.equal(outs[5, top:top + h], ins[5]) and torch.equal(outs[5, top + h:], want))
+    row("expand_64x3840x2160_to_3840x2880_one_call", ms, n * (4 * w * H + 4 * w * h), frames=n, spot_check_ok=ok)
+    del ins, outs, iw, ow, ops
+    torch.cuda.empty_cache()
+
+    # padded thumbnails: 1024 x 512x288 -> 512x512, one call and 1024 calls
+    n, w, h, H = 1024, 512, 288, 512
+    ins = torch.randint(0, 256, (n, h, w, 4), dtype=torch.uint8, device="cuda")
+    outs = torch.empty((n, H, w, 4), dtype=torch.uint8, device="cuda")
+    top = (H - h) // 2
+    ops = [ifb.ExpandCanvas(ifb.BitmapWindow.from_torch(ins[i]), 0, top, 0, H - h - top, (255, 255, 255, 255),
+                            canvas=ifb.BitmapWindow.from_torch(outs[i])) for i in range(n)]
+    alg = n * (4 * w * H + 4 * w * h)
+    row("pad_1024x512x288_to_512x512_one_call", _time_ms(lambda: b.canvas(ops, stream)), alg, frames=n)
+    row("pad_1024x512x288_to_512x512_1024_calls", _time_ms(lambda: [b.canvas([o], stream) for o in ops], reps=3), alg, frames=n)
+    ok = bool(torch.equal(outs[7, top:top + h], ins[7]))
+    # WatermarkRedDot on the 1024 padded frames
+    dots = [op for i in range(n) for op in ifb.watermark_red_dot(ifb.BitmapWindow.from_torch(outs[i]))]
+    row("red_dot_1024_frames_one_call", _time_ms(lambda: b.canvas(dots, stream)), n * 9 * 4, frames=n, spot_check_ok=ok)
+    row("red_dot_1024_frames_1024_calls", _time_ms(lambda: [b.canvas([o], stream) for o in dots], reps=3), n * 9 * 4, frames=n)
+    del ins, outs, ops, dots
+    torch.cuda.empty_cache()
+
+    # mode=pad at config 2 (3840x2160 -> 512x288 Robidoux, linear light, then 512x512): (a) resample + EXPAND, (b) resample into the
+    # interior + border FILL_RECTs.  The rows time the whole pipeline; bytes are the resample's (4K read, 512x288 written) plus the pad's.
+    n = 64
+    ins = (torch.randn((n, 2160, 3840, 4), device="cuda") * 40 + 128).clamp_(0, 255).to(torch.uint8)
+    mid = torch.empty((n, 288, 512, 4), dtype=torch.uint8, device="cuda")
+    pa = torch.empty((n, 512, 512, 4), dtype=torch.uint8, device="cuda")
+    pb = torch.empty((n, 512, 512, 4), dtype=torch.uint8, device="cuda")
+    params = ifb.ScaleAndRenderParams(w=512, h=288)
+    srcs = [ifb.BitmapWindow.from_torch(ins[i]) for i in range(n)]
+    mids = [ifb.BitmapWindow.from_torch(mid[i]) for i in range(n)]
+    descs_a, keep_a = b.make_descs([(srcs[i], mids[i], params) for i in range(n)])
+    exp_a = [ifb.ExpandCanvas(mids[i], 0, 112, 0, 112, (9, 99, 199, 77), canvas=ifb.BitmapWindow.from_torch(pa[i])) for i in range(n)]
+    descs_b, keep_b = b.make_descs([(srcs[i], ifb.BitmapWindow.from_torch(pb[i]).window(0, 112, 512, 400), params) for i in range(n)])
+    fills_b = [f for i in range(n) for f in (ifb.FillRect(ifb.BitmapWindow.from_torch(pb[i]), 0, 0, 512, 112, (9, 99, 199, 77)),
+                                             ifb.FillRect(ifb.BitmapWindow.from_torch(pb[i]), 0, 400, 512, 512, (9, 99, 199, 77)))]
+    route_a = lambda: (b.enqueue(descs_a, stream), b.canvas(exp_a, stream))
+    route_b = lambda: (b.enqueue(descs_b, stream), b.canvas(fills_b, stream))
+    base = n * (3840 * 2160 * 4)
+    ms_a, ms_b = _time_ms(route_a), _time_ms(route_b)
+    same = bool(torch.equal(pa, pb))
+    row("mode_pad_config2_route_a_resample_then_expand", ms_a, base + n * (288 * 512 * 4 + 512 * 512 * 4 + 288 * 512 * 4), frames=n,
+        routes_agree=same)
+    row("mode_pad_config2_route_b_resample_into_interior_then_fill", ms_b, base + n * 512 * 512 * 4, frames=n, routes_agree=same)
+    b.sync()
+
+
 if __name__ == "__main__":
-    main()
+    if sys.argv[1:] == ["canvas"]:
+        canvas_rows()
+    else:
+        main()
