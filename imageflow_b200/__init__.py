@@ -12,6 +12,8 @@ Host-side mirror of the reference seam (paths relative to the imageflow checkout
   graphics/rounded_corners.rs:187  flow_bitmap_bgra_clear_around_rounded_corners, RoundCornersMode (imageflow_types)
   graphics/bitmaps.rs:1504,1570, graphics/copy_rect.rs:12  fill_rectangle, normalize_unused_alpha, copy_rectangle (Batch.canvas:
       FillRect, EnableTransparency, CopyRectToCanvas, ExpandCanvas; WatermarkRedDot, Region, RegionPercent as helpers)
+  flow/nodes/rotate_flip_transpose.rs  ApplyOrientation, Rotate90/180/270, FlipH, FlipV, Transpose as one gather (Batch.orient,
+      orientation_of; RIAPI's add_rotate / add_flip as riapi_rotate_steps / riapi_flip_steps)
   c_components/lib/codecs_jpeg_idct_fast.c  flow_scale_spatial[_srgb]_NxN (decode-time JPEG block scalers)
 All arithmetic runs in hand-written sm_90a kernels inside libifb200.so (include/ifb200.h);
 this package only marshals arguments.  Nothing here imports the CPU oracle.
@@ -21,7 +23,9 @@ from .graphics import (Batch, apply_matte, BitmapCompositing, BitmapWindow, Erro
                        window_bgra32_apply_color_matrix, bitmap_window_transpose, flow_bitmap_bgra_flip_vertical_safe,
                        flow_bitmap_bgra_flip_horizontal_safe, white_balance_srgb_mut, detect_content, detect_content_from_codes, flow_scale_spatial,
                        RoundCornersMode, flow_bitmap_bgra_clear_around_rounded_corners,
-                       FillRect, CopyRectToCanvas, ExpandCanvas, EnableTransparency, new_canvas, watermark_red_dot, region, region_percent)
+                       FillRect, CopyRectToCanvas, ExpandCanvas, EnableTransparency, new_canvas, watermark_red_dot, region, region_percent,
+                       ApplyOrientation, Rotate90, Rotate180, Rotate270, FlipH, FlipV, Transpose, orientation_of, riapi_rotate_steps,
+                       riapi_flip_steps, apply_orientation)
 from ._lib import LIB_PATH, ResampleDesc, lib
 
 __all__ = [
@@ -30,5 +34,7 @@ __all__ = [
     "window_bgra32_apply_color_matrix", "bitmap_window_transpose", "flow_bitmap_bgra_flip_vertical_safe",
     "flow_bitmap_bgra_flip_horizontal_safe", "white_balance_srgb_mut", "detect_content", "detect_content_from_codes", "flow_scale_spatial",
     "RoundCornersMode", "flow_bitmap_bgra_clear_around_rounded_corners",
-    "FillRect", "CopyRectToCanvas", "ExpandCanvas", "EnableTransparency", "new_canvas", "watermark_red_dot", "region", "region_percent", "LIB_PATH", "ResampleDesc", "lib",
+    "FillRect", "CopyRectToCanvas", "ExpandCanvas", "EnableTransparency", "new_canvas", "watermark_red_dot", "region", "region_percent",
+    "ApplyOrientation", "Rotate90", "Rotate180", "Rotate270", "FlipH", "FlipV", "Transpose", "orientation_of", "riapi_rotate_steps",
+    "riapi_flip_steps", "apply_orientation", "LIB_PATH", "ResampleDesc", "lib",
 ]

@@ -21,7 +21,7 @@ SYMBOLS = [
     "ifb200_batch_destroy", "ifb200_batch_set_option", "ifb200_batch_kernel_launches", "ifb200_batch_host_profile",
     "ifb200_batch_fused_jobs", "ifb200_batch_generic_jobs", "ifb200_batch_tile_jobs", "ifb200_batch_ring_status", "ifb200_hv_plan_tables",
     "ifb200_block_scale_u8", "ifb200_batch_block_scale", "ifb200_round_corners_bgra8", "ifb200_batch_round_corners",
-    "ifb200_batch_canvas",
+    "ifb200_batch_canvas", "ifb200_batch_orient",
 ]
 
 
@@ -53,6 +53,14 @@ class CanvasDesc(C.Structure):
         ("in_", C.c_void_p), ("in_w", C.c_uint32), ("in_h", C.c_uint32), ("in_stride", C.c_uint32), ("in_alpha_meaningful", C.c_int32),
         ("x1", C.c_uint32), ("y1", C.c_uint32), ("x2", C.c_uint32), ("y2", C.c_uint32), ("cw", C.c_uint32), ("ch", C.c_uint32),
         ("color_bgra", C.c_uint8 * 4),
+    ]
+
+
+class OrientDesc(C.Structure):
+    """struct ifb200_orient_desc"""
+    _fields_ = [
+        ("in_", C.c_void_p), ("in_w", C.c_uint32), ("in_h", C.c_uint32), ("in_stride", C.c_uint32),
+        ("out", C.c_void_p), ("out_stride", C.c_uint32), ("orientation", C.c_int32),
     ]
 
 
@@ -144,6 +152,8 @@ def lib() -> C.CDLL:
     L.ifb200_batch_round_corners.restype = C.c_int
     L.ifb200_batch_canvas.argtypes = [C.c_void_p, C.POINTER(CanvasDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_canvas.restype = C.c_int
+    L.ifb200_batch_orient.argtypes = [C.c_void_p, C.POINTER(OrientDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
+    L.ifb200_batch_orient.restype = C.c_int
     L.ifb200_batch_ring_status.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_ring_status.restype = C.c_int
     _lib = L

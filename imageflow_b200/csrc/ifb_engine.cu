@@ -1267,6 +1267,28 @@ void canvas_locked(ifb200_batch* b, const ifb200_canvas_desc* d, size_t n, cudaS
     b->launches++;
 }
 
+// The orientations of ifb200_batch_orient (ifb_orient.h): every descriptor is checked before anything is planned or enqueued, then
+// all jobs run in ONE launch (none when no job writes a pixel).  The upload is the items and their first CTAs, O(jobs).
+void orient_locked(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    for (size_t i = 0; i < n; ++i) {
+        const std::string why = ifb::orient_check(d[i]);
+        if (!why.empty()) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "orient job %zu: %s", i, why.c_str());
+    }
+    ifb::OrWork wk;
+    for (size_t i = 0; i < n; ++i) ifb::orient_plan(d[i], wk);
+    if (wk.items.empty()) return;
+    if (wk.ctas() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
+    DeviceScope dev_scope_(b->device);
+    size_t fb = 0;
+    uint8_t* dbuf = upload_work(b, wk.items, wk.first, st, &fb);
+    AsyncFree dbuf_guard{dbuf, st};
+    orient_kernel<<<(unsigned)wk.ctas(), ifb::kOrThreads, 0, st>>>(reinterpret_cast<const ifb::OrItem*>(dbuf),
+                                                                 reinterpret_cast<const uint32_t*>(dbuf + fb), (uint32_t)wk.items.size());
+    CUDA_OK(cudaGetLastError());
+    b->launches++;
+}
+
 // Pageable host bitmaps (imageflow's Bitmap buffers are plain Vecs, aligned_buffer.rs:40-43): cudaMemcpy2DAsync from pageable memory
 // is staged by the driver on the calling thread (about 10 GB/s, and it does not overlap).  The drop-in path therefore stages such
 // bitmaps itself: the rows are copied into a pinned buffer of the pipeline slot by a few host threads in parallel, the pinned buffer
@@ -1651,6 +1673,14 @@ int ifb200_batch_canvas(ifb200_batch* b, const ifb200_canvas_desc* d, size_t n, 
         if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
         std::lock_guard<std::mutex> lk(b->mu);
         canvas_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
+    });
+}
+
+int ifb200_batch_orient(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, void* stream, char* err, size_t cap) {
+    return guarded(err, cap, [&] {
+        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
+        std::lock_guard<std::mutex> lk(b->mu);
+        orient_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
     });
 }
 

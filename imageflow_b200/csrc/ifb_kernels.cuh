@@ -20,6 +20,7 @@
 
 #include "ifb_round_corners.h"     // RcJob / RcTile: planned on the host, read by round_corners_kernel
 #include "ifb_canvas.h"            // CvItem / CvTile: planned on the host, read by canvas_kernel
+#include "ifb_orient.h"            // OrItem: planned on the host, read by orient_kernel
 
 namespace ifbk {
 
@@ -355,6 +356,9 @@ __global__ void __launch_bounds__(256) apply_byte_maps_bgra8_kernel(uint8_t* __r
 
 // ---------------------------------------------------------------- canvas operations (fill, copy, expand, normalise alpha); own file for tests/cpu_emu
 #include "ifb_canvas_kernel.cuh"
+
+// ---------------------------------------------------------------- orientation (ApplyOrientation, rotations, flips, transpose) as one gather; own file for tests/cpu_emu
+#include "ifb_orient_kernel.cuh"
 
 // ---------------------------------------------------------------- decode-time JPEG block scalers (SURVEY.md section 8(f), item 1)
 #include "ifb_idct_kernel.cuh"

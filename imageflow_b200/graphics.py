@@ -9,7 +9,7 @@ from typing import Optional, Sequence
 
 import numpy as np
 
-from ._lib import CanvasDesc, ResampleDesc, RoundCornersDesc, lib
+from ._lib import CanvasDesc, OrientDesc, ResampleDesc, RoundCornersDesc, lib
 
 
 class Filter(enum.IntEnum):
@@ -410,6 +410,87 @@ def _fill_canvas_desc(d: CanvasDesc, op, device: int):
     raise FlowError(ErrorKind.InvalidArgument, f"not a canvas operation: {op!r}")
 
 
+# ---------------------------------------------------------------- orientation (Batch.orient), named after the imageflow_types nodes
+@dataclass(frozen=True)
+class ApplyOrientation:
+    """Node::ApplyOrientation { flag }: the EXIF orientation a decoder inserts after the decode (flow/nodes/codecs_and_pointer.rs)."""
+    flag: int
+
+
+# the unit nodes of imageflow_types
+Rotate90, Rotate180, Rotate270, FlipH, FlipV, Transpose = "Rotate90", "Rotate180", "Rotate270", "FlipH", "FlipV", "Transpose"
+
+# the reference's expansions (flow/nodes/rotate_flip_transpose.rs): ApplyOrientation by flag (any other flag: nothing), then the
+# rotations into flips and transposes
+_APPLY_ORIENTATION = {2: (FlipH,), 3: (Rotate180,), 4: (FlipV,), 5: (Transpose,), 6: (Rotate90,), 7: (Rotate180, Transpose), 8: (Rotate270,)}
+_EXPANSION = {Rotate90: (FlipV, Transpose), Rotate180: (FlipV, FlipH), Rotate270: (Transpose, FlipV),
+              FlipH: (FlipH,), FlipV: (FlipV,), Transpose: (Transpose,)}
+# EXIF orientation -> (transposes, source x reversed, source y reversed): out(x, y) = in(x', y') as in include/ifb200.h
+_ORIENTATION = {1: (False, False, False), 2: (False, True, False), 3: (False, True, True), 4: (False, False, True),
+                5: (True, False, False), 6: (True, False, True), 7: (True, True, True), 8: (True, True, False)}
+
+
+_ORIENT_DESC_DTYPE = np.dtype({"names": [n for n, _ in OrientDesc._fields_],
+                               "formats": [np.uint64 if t is C.c_void_p else np.dtype(t) for n, t in OrientDesc._fields_],
+                               "offsets": [getattr(OrientDesc, n).offset for n, _ in OrientDesc._fields_], "itemsize": C.sizeof(OrientDesc)})
+
+
+def _primitives(steps):
+    for s in steps:
+        if isinstance(s, ApplyOrientation):
+            yield from _primitives(_APPLY_ORIENTATION.get(int(s.flag), ()))
+        elif s in _EXPANSION:
+            yield from _EXPANSION[s]
+        else:
+            raise FlowError(ErrorKind.InvalidArgument, f"not an orientation node: {s!r}")
+
+
+def _oriented(a: np.ndarray, orientation: int) -> np.ndarray:
+    """the output of `orientation` on a (rows, columns) array, as a view"""
+    t, fx, fy = _ORIENTATION.get(int(orientation), _ORIENTATION[1])
+    b = a[::-1 if fy else 1, ::-1 if fx else 1]
+    return b.swapaxes(0, 1) if t else b
+
+
+def orientation_of(steps) -> int:
+    """The EXIF orientation 1..8 that a chain of ApplyOrientation(flag), Rotate90, Rotate180, Rotate270, FlipH, FlipV and Transpose
+    nodes amounts to: every such chain is one element of the eight symmetries of a rectangle, found here by its action on a 3 x 2
+    probe."""
+    probe = np.arange(6).reshape(2, 3)
+    a = probe
+    for p in _primitives(steps):
+        a = a[:, ::-1] if p == FlipH else a[::-1] if p == FlipV else a.T
+    return next(o for o in range(1, 9) if np.array_equal(_oriented(probe, o), a))
+
+
+def _rust_div_rem(a: int, b: int):
+    """Rust's i32 `/` (truncating) and `%` (the sign of a)"""
+    q = abs(a) // abs(b) * (1 if (a >= 0) == (b >= 0) else -1)
+    return q, a - b * q
+
+
+def riapi_rotate_steps(degrees: int) -> list:
+    """add_rotate of RIAPI's layout (imageflow_riapi ir4/layout.rs) for `rotate=` / `srotate=`: match ((rot / 90) + 4) % 4 in i32,
+    so -90 is Rotate270, 45 nothing, and -450 nothing (the remainder -1 matches no arm)."""
+    q, _ = _rust_div_rem(int(degrees), 90)
+    _, r = _rust_div_rem(q + 4, 4)
+    return [{1: Rotate90, 2: Rotate180, 3: Rotate270}[r]] if r in (1, 2, 3) else []
+
+
+def riapi_flip_steps(h: bool, v: bool) -> list:
+    """add_flip of RIAPI's layout for `flip=` / `sflip=` as (h, v): FlipH, then FlipV."""
+    return ([FlipH] if h else []) + ([FlipV] if v else [])
+
+
+def apply_orientation(window: BitmapWindow, flag: int, device: int = 0):
+    """The job of Batch.orient for ApplyOrientation { flag } of `window` into a newly allocated canvas of the window's format (its
+    dimensions swapped for 5..8, rows padded to 64 bytes as bitmaps.rs:803-804): (window, canvas, flag).  Batch.orient returns the
+    canvas."""
+    t = _ORIENTATION.get(int(flag), _ORIENTATION[1])[0]
+    w, h = (window.h, window.w) if t else (window.w, window.h)
+    return window, new_canvas(w, h, _device_of(window, device), window.alpha_meaningful), int(flag)
+
+
 def flow_scale_spatial(samples: np.ndarray, n: int, srgb: bool = False) -> np.ndarray:
     """flow_scale_spatial[_srgb]_{n}x{n} (c_components/lib/codecs_jpeg_idct_fast.c) applied to every 8x8 block of a plane of
     samples (H x W uint8, both multiples of 8; host memory): returns the (H/8*n) x (W/8*n) plane."""
@@ -610,6 +691,33 @@ class Batch:
         out = [f() for f in done]
         self._keep.append([[getattr(op, n, None) for n in ("window", "input", "canvas")] for op in ops] + [w._keep for w in out])
         return out
+
+    def orient(self, jobs, stream=None) -> list:
+        """EXIF orientations on DEVICE windows, one read and one write per pixel, all jobs in one kernel launch (none when no job
+        writes a pixel), asynchronous on `stream`.  jobs: iterable of (input, output or None for in place, orientation); compose a
+        chain of nodes into one orientation with orientation_of().  The output is w x h for 1..4 and h x w for 5..8; in place needs
+        1..4.  No job may write what another job of the call reads or writes.  Returns the output windows (with the input's
+        alpha_meaningful); nothing is changed when an argument is rejected."""
+        jobs = list(jobs)
+        outs = []
+        for inp, out, o in jobs:
+            out = inp if out is None else out
+            t = _ORIENTATION.get(int(o), _ORIENTATION[1])[0]
+            if (out.w, out.h) != ((inp.h, inp.w) if t else (inp.w, inp.h)) or inp.pixel_layout != "BGRA" or out.pixel_layout != "BGRA":
+                raise FlowError(ErrorKind.InvalidArgument, f"orientation {o} of a {inp.w}x{inp.h} BGRA window needs a "
+                                                           f"{'%dx%d' % ((inp.h, inp.w) if t else (inp.w, inp.h))} BGRA output, not {out.w}x{out.h}")
+            outs.append(out)
+        a = np.zeros(len(jobs), _ORIENT_DESC_DTYPE)               # filled a column at a time: no per-field ctypes marshalling
+        a["in_"] = [j[0].ptr for j in jobs]; a["in_w"] = [j[0].w for j in jobs]; a["in_h"] = [j[0].h for j in jobs]
+        a["in_stride"] = [j[0].stride for j in jobs]; a["out"] = [o.ptr for o in outs]; a["out_stride"] = [o.stride for o in outs]
+        a["orientation"] = [int(j[2]) for j in jobs]
+        arr = (OrientDesc * len(jobs)).from_buffer(a)
+        buf = C.create_string_buffer(512)
+        _check(lib().ifb200_batch_orient(self._h, arr, len(jobs), self._stream(stream), buf, 512), buf)
+        for (inp, _, _), out in zip(jobs, outs):
+            out.alpha_meaningful = inp.alpha_meaningful
+        self._keep.append([(j[0]._keep, o._keep) for j, o in zip(jobs, outs)])
+        return outs
 
     def flip_vertical(self, bitmap: BitmapWindow, stream=None) -> None:
         """graphics/flip.rs:10-22 on a DEVICE bitmap, in place."""

@@ -203,6 +203,19 @@ typedef struct ifb200_canvas_desc {
     uint8_t  color_bgra[4];    /* FILL / EXPAND: Color::to_bgra8() */
 } ifb200_canvas_desc;
 
+/* One orientation job: ApplyOrientation { flag } (flow/nodes/rotate_flip_transpose.rs:50-66) and every chain of Rotate90 / 180 /
+ * 270, FlipH, FlipV and Transpose, which compose into one of the eight EXIF orientations.  With the input window w x h, the output
+ * is w x h for 1..4 and h x w for 5..8, and out(x, y) = in(...) with
+ *   1 (x, y)   2 (w-1-x, y)   3 (w-1-x, h-1-y)   4 (x, h-1-y)   5 (y, x)   6 (y, h-1-x)   7 (w-1-y, h-1-x)   8 (w-1-y, x)
+ * Pixels move as raw 4-byte words, alpha included.  Any flag other than 2..8 is the identity, as the reference's `_ => vec![]`.
+ * out == in (same pointer and stride) is in place, allowed for 1..4 only (the reference panics on an in-place transpose,
+ * :158-160); otherwise the input and output byte spans must not overlap.  A job of zero area is skipped unchecked. */
+typedef struct ifb200_orient_desc {
+    const uint8_t* in;  uint32_t in_w, in_h, in_stride;   /* BGRA8 window; stride in bytes */
+    uint8_t*       out; uint32_t out_stride;              /* in_w x in_h for 1..4, in_h x in_w for 5..8; may equal `in` for 1..4 */
+    int32_t        orientation;                           /* EXIF flag; values other than 2..8 are the identity */
+} ifb200_orient_desc;
+
 /* ---- device-resident batch API (the metric path; not in the reference) -----------------------
  * descs[i].in / .canvas are DEVICE pointers on the batch's device; color_matrix stays a HOST pointer.
  * enqueue is asynchronous on `cuda_stream`, a cudaStream_t with the usual CUDA meaning (NULL = the legacy
@@ -249,6 +262,11 @@ int  ifb200_batch_round_corners(ifb200_batch* b, const ifb200_round_corners_desc
  * overlap in memory.  Argument errors are reported before anything is enqueued.  There is no host-buffer variant: on a host bitmap
  * these ops are a memset / memcpy, cheaper than a trip to the GPU. */
 int  ifb200_batch_canvas(ifb200_batch* b, const ifb200_canvas_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
+/* Orientation (ifb200_orient_desc) of n DEVICE windows in ONE kernel launch, one read and one write per pixel whatever the flag;
+ * none when no job writes a pixel (the identity in place, zero-area jobs).  Asynchronous on `cuda_stream`.  No job may write what
+ * another job of the same call reads or writes (not checked).  Argument errors are reported before anything is enqueued.  There is
+ * no host-buffer variant: on a host bitmap the reference's own transpose beats a trip to the GPU. */
+int  ifb200_batch_orient(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
 int  ifb200_batch_sync(ifb200_batch* b, char* err, size_t err_cap);
 void ifb200_batch_destroy(ifb200_batch* b);
 /* knobs / introspection (benchmarks, tests) */

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Measurement of the SURVEY.md section 8(f) neighbours of the resample path that are built: transpose, flips, white balance, detect_content
-and rounded corners; `bench_neighbours.py canvas` measures the canvas operations alone (canvas_rows)
+and rounded corners; `bench_neighbours.py canvas` measures the canvas operations alone (canvas_rows), `bench_neighbours.py orient`
+the one-gather orientation against the reference's expansion into transposes and flips (orient_rows)
 (the reference benchmarks transposes at 4K / 8K in benches/bench_graphics.rs:9-62).  Inputs resident in HBM, CUDA events on
 the launching stream, >= 3 warm-up calls; a set of 64 different images per size (>= 2 GB, far larger than L2) is cycled so that
 no call finds its data in cache.  One JSON line per (operation, size) with the HBM roofline of the kernel: algorithmic
@@ -280,8 +281,101 @@ def canvas_rows():
     b.sync()
 
 
+def _time_event_and_host_ms(fn, reps=10):
+    """(CUDA-event time on the current stream, host wall time spent inside fn) per call of fn, after 3 warm-up calls"""
+    for _ in range(3):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    host = 0.0
+    e0.record()
+    for _ in range(reps):
+        t0 = time.perf_counter()
+        fn()
+        host += time.perf_counter() - t0
+    e1.record(); torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / reps, host * 1e3 / reps
+
+
+def orient_rows():
+    """Orientation (Batch.orient) on frames resident in HBM: 64 3840x2160 frames in one call for each of flags 2..8, against the
+    reference's expansion of the same flag with the existing single-window transpose and flip calls (one launch and one full pass per
+    node, in place for the flips, as the reference runs them), and against a torch device-to-device copy of the same bytes.
+    Algorithmic bytes: 4 read + 4 written per pixel; the 64 frames (2.1 GB) are cycled, far larger than L2.  Then 1024 512x384
+    thumbnails in one call and as 1024 calls, with the CUDA-event time on the stream and the host wall time of the calls apart."""
+    from tests import orient_oracle as oo
+    card = _card()
+    pk, src = peak()
+    b = ifb.Batch(0)
+    stream = torch.cuda.current_stream().cuda_stream
+
+    def row(name, ms, alg, **kw):
+        cm = _copy_ceiling_ms(alg)
+        print(json.dumps({"op": "orient", "row": name, "ms": ms, "algorithmic_bytes": alg, "achieved_gbs": alg / ms / 1e6,
+                          "frac_of_peak": alg / ms / 1e6 / pk, "peak_gbs": pk, "peak_source": src, "torch_copy_same_bytes_ms": cm,
+                          "frac_of_torch_copy": cm / ms, **kw, **card}), flush=True)
+
+    n, w, h = 64, 3840, 2160
+    ins = torch.randint(0, 256, (n, h, w, 4), dtype=torch.uint8, device="cuda")
+    same = torch.empty((n, h, w, 4), dtype=torch.uint8, device="cuda")
+    swapped = torch.empty((n, w, h, 4), dtype=torch.uint8, device="cuda")
+    iw = [ifb.BitmapWindow.from_torch(ins[i]) for i in range(n)]
+    sw = [ifb.BitmapWindow.from_torch(same[i]) for i in range(n)]
+    tw = [ifb.BitmapWindow.from_torch(swapped[i]) for i in range(n)]
+    alg = n * w * h * 8
+
+    def expansion(i, flag):
+        """ApplyOrientation(flag) of frame i node by node (the flips in place on the frame, the transpose into `swapped`)"""
+        cur, t = iw[i], False
+        for p in oo.primitives([("ApplyOrientation", flag)]):
+            if p == oo.TRANSPOSE:
+                b.transpose(cur, tw[i], stream); cur, t = tw[i], True
+            else:
+                (b.flip_horizontal if p == oo.FLIP_H else b.flip_vertical)(cur, stream)
+        return t
+
+    for flag in range(2, 9):
+        t = flag >= 5
+        outs = tw if t else sw
+        jobs = [(iw[i], outs[i], flag) for i in range(n)]
+        ms_one = _time_ms(lambda: b.orient(jobs, stream))
+        nodes = len(oo.primitives([("ApplyOrientation", flag)]))
+        ms_exp = _time_ms(lambda: [expansion(i, flag) for i in range(n)])
+        # bit-exactness of frame 0: the one call against the expansion on a copy
+        keep = ins[0].clone()
+        b.orient([(iw[0], outs[0], flag)], stream)
+        got = (swapped if t else same)[0].clone()
+        expansion(0, flag)
+        want = swapped[0].clone() if t else ins[0].clone()
+        ins[0].copy_(keep)
+        ok = bool(torch.equal(got, want))
+        kw = dict(flag=flag, frames=n, size=f"{w}x{h}", expansion_nodes=nodes, expansion_ms=ms_exp, one_call_vs_expansion=ms_exp / ms_one,
+                  bit_exact_vs_expansion=ok)
+        if not t:
+            kw["in_place_ms"] = _time_ms(lambda: b.orient([(iw[i], None, flag) for i in range(n)], stream))
+        row(f"flag{flag}_64x{w}x{h}_one_call", ms_one, alg, **kw)
+    del ins, same, swapped, iw, sw, tw
+    torch.cuda.empty_cache()
+
+    # thumbnails: 1024 x 512x384 with flag 6, one call and 1024 calls
+    n, w, h = 1024, 512, 384
+    ins = torch.randint(0, 256, (n, h, w, 4), dtype=torch.uint8, device="cuda")
+    outs = torch.empty((n, w, h, 4), dtype=torch.uint8, device="cuda")
+    jobs = [(ifb.BitmapWindow.from_torch(ins[i]), ifb.BitmapWindow.from_torch(outs[i]), 6) for i in range(n)]
+    alg = n * w * h * 8
+    ev, host = _time_event_and_host_ms(lambda: b.orient(jobs, stream))
+    row("flag6_1024x512x384_one_call", ev, alg, frames=n, host_wall_ms=host)
+    ev, host = _time_event_and_host_ms(lambda: [b.orient([j], stream) for j in jobs], reps=3)
+    row("flag6_1024x512x384_1024_calls", ev, alg, frames=n, host_wall_ms=host)
+    want = torch.from_numpy(oo.gather(ins[7].cpu().numpy(), 6)).cuda()
+    print(json.dumps({"op": "orient", "row": "thumbnail_spot_check", "bit_exact_vs_closed_form": bool(torch.equal(outs[7], want)), **card}))
+    b.sync()
+
+
 if __name__ == "__main__":
     if sys.argv[1:] == ["canvas"]:
         canvas_rows()
+    elif sys.argv[1:] == ["orient"]:
+        orient_rows()
     else:
         main()
