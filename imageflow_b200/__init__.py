@@ -14,6 +14,8 @@ Host-side mirror of the reference seam (paths relative to the imageflow checkout
       FillRect, EnableTransparency, CopyRectToCanvas, ExpandCanvas; WatermarkRedDot, Region, RegionPercent as helpers)
   flow/nodes/rotate_flip_transpose.rs  ApplyOrientation, Rotate90/180/270, FlipH, FlipV, Transpose as one gather (Batch.orient,
       orientation_of; RIAPI's add_rotate / add_flip as riapi_rotate_steps / riapi_flip_steps)
+  flow/nodes/color.rs, enable_transparency.rs, white_balance.rs  ColorMatrixSrgb, ColorFilterSrgb presets, EnableTransparency and
+      WhiteBalanceHistogramAreaThresholdSrgb as one chain per frame (Batch.color_chain; RIAPI's s.* / a.balancewhite as riapi_color_steps)
   c_components/lib/codecs_jpeg_idct_fast.c  flow_scale_spatial[_srgb]_NxN (decode-time JPEG block scalers)
 All arithmetic runs in hand-written sm_90a kernels inside libifb200.so (include/ifb200.h);
 this package only marshals arguments.  Nothing here imports the CPU oracle.
@@ -25,7 +27,8 @@ from .graphics import (Batch, apply_matte, BitmapCompositing, BitmapWindow, Erro
                        RoundCornersMode, flow_bitmap_bgra_clear_around_rounded_corners,
                        FillRect, CopyRectToCanvas, ExpandCanvas, EnableTransparency, new_canvas, watermark_red_dot, region, region_percent,
                        ApplyOrientation, Rotate90, Rotate180, Rotate270, FlipH, FlipV, Transpose, orientation_of, riapi_rotate_steps,
-                       riapi_flip_steps, apply_orientation)
+                       riapi_flip_steps, apply_orientation, ColorMatrixSrgb, ColorFilterSrgb, WhiteBalanceHistogramAreaThresholdSrgb,
+                       riapi_color_steps)
 from ._lib import LIB_PATH, ResampleDesc, lib
 
 __all__ = [
@@ -36,5 +39,6 @@ __all__ = [
     "RoundCornersMode", "flow_bitmap_bgra_clear_around_rounded_corners",
     "FillRect", "CopyRectToCanvas", "ExpandCanvas", "EnableTransparency", "new_canvas", "watermark_red_dot", "region", "region_percent",
     "ApplyOrientation", "Rotate90", "Rotate180", "Rotate270", "FlipH", "FlipV", "Transpose", "orientation_of", "riapi_rotate_steps",
-    "riapi_flip_steps", "apply_orientation", "LIB_PATH", "ResampleDesc", "lib",
+    "riapi_flip_steps", "apply_orientation", "ColorMatrixSrgb", "ColorFilterSrgb", "WhiteBalanceHistogramAreaThresholdSrgb",
+    "riapi_color_steps", "LIB_PATH", "ResampleDesc", "lib",
 ]

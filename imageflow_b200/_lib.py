@@ -21,7 +21,7 @@ SYMBOLS = [
     "ifb200_batch_destroy", "ifb200_batch_set_option", "ifb200_batch_kernel_launches", "ifb200_batch_host_profile",
     "ifb200_batch_fused_jobs", "ifb200_batch_generic_jobs", "ifb200_batch_tile_jobs", "ifb200_batch_ring_status", "ifb200_hv_plan_tables",
     "ifb200_block_scale_u8", "ifb200_batch_block_scale", "ifb200_round_corners_bgra8", "ifb200_batch_round_corners",
-    "ifb200_batch_canvas", "ifb200_batch_orient",
+    "ifb200_batch_canvas", "ifb200_batch_orient", "ifb200_batch_color_chain",
 ]
 
 
@@ -61,6 +61,19 @@ class OrientDesc(C.Structure):
     _fields_ = [
         ("in_", C.c_void_p), ("in_w", C.c_uint32), ("in_h", C.c_uint32), ("in_stride", C.c_uint32),
         ("out", C.c_void_p), ("out_stride", C.c_uint32), ("orientation", C.c_int32),
+    ]
+
+
+class ColorStep(C.Structure):
+    """struct ifb200_color_step"""
+    _fields_ = [("kind", C.c_int32), ("matrix", C.c_float * 25), ("threshold", C.c_float)]
+
+
+class ColorDesc(C.Structure):
+    """struct ifb200_color_desc"""
+    _fields_ = [
+        ("px", C.c_void_p), ("w", C.c_uint32), ("h", C.c_uint32), ("stride", C.c_uint32), ("alpha_meaningful", C.c_int32),
+        ("steps", C.c_void_p), ("n_steps", C.c_uint32),
     ]
 
 
@@ -154,6 +167,8 @@ def lib() -> C.CDLL:
     L.ifb200_batch_canvas.restype = C.c_int
     L.ifb200_batch_orient.argtypes = [C.c_void_p, C.POINTER(OrientDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_orient.restype = C.c_int
+    L.ifb200_batch_color_chain.argtypes = [C.c_void_p, C.POINTER(ColorDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
+    L.ifb200_batch_color_chain.restype = C.c_int
     L.ifb200_batch_ring_status.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_ring_status.restype = C.c_int
     _lib = L

@@ -1289,6 +1289,60 @@ void orient_locked(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, cudaS
     b->launches++;
 }
 
+// The colour chains of ifb200_batch_color_chain (ifb_color.h): every descriptor is checked before anything is planned or enqueued.
+// The plan (jobs, prefix sums, segments, tables, matrices) goes up in one copy, O(jobs + steps); then ONE launch, or three when some
+// job white-balances (histograms into zeroed counters, byte maps into the jobs' kClWb tables, apply); none when no job writes a pixel.
+void color_chain_locked(ifb200_batch* b, const ifb200_color_desc* d, size_t n, cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    for (size_t i = 0; i < n; ++i) {
+        int code = 0;
+        const std::string why = ifb::color_check(d[i], &code);
+        if (!why.empty()) IFB_THROW(code, "color job %zu: %s", i, why.c_str());
+    }
+    ifb::ClWork wk;
+    for (size_t i = 0; i < n; ++i) ifb::color_plan(d[i], wk);
+    if (wk.jobs.empty()) return;
+    if (wk.ctas() > 0x7fffffffu || wk.wb_ctas() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
+    DeviceScope dev_scope_(b->device);
+    auto at = [](size_t x) { return (x + 255) / 256 * 256; };
+    const size_t o_first = at(wk.jobs.size() * sizeof(ifb::ClJob)), o_wb = o_first + at(wk.first.size() * 4),
+                 o_wbf = o_wb + at(wk.wb_jobs.size() * sizeof(ifb::ClJob)), o_segs = o_wbf + at(wk.wb_first.size() * 4),
+                 o_tab = o_segs + at(wk.segs.size() * sizeof(ifb::ClSeg)), o_mat = o_tab + at(wk.tables.size()),
+                 o_hist = o_mat + at(wk.mats.size() * sizeof(float)), hist_bytes = wk.wb_jobs.size() * 768 * sizeof(unsigned long long);
+    cudaEvent_t ev;
+    uint8_t* h = static_cast<uint8_t*>(b->stage(o_hist, &ev));
+    auto put = [&](size_t off, const void* src, size_t bytes) { if (bytes) memcpy(h + off, src, bytes); };
+    put(0, wk.jobs.data(), wk.jobs.size() * sizeof(ifb::ClJob));
+    put(o_first, wk.first.data(), wk.first.size() * 4);
+    put(o_wb, wk.wb_jobs.data(), wk.wb_jobs.size() * sizeof(ifb::ClJob));
+    put(o_wbf, wk.wb_first.data(), wk.wb_first.size() * 4);
+    put(o_segs, wk.segs.data(), wk.segs.size() * sizeof(ifb::ClSeg));
+    put(o_tab, wk.tables.data(), wk.tables.size());
+    put(o_mat, wk.mats.data(), wk.mats.size() * sizeof(float));
+    uint8_t* dbuf = nullptr;
+    CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&dbuf), o_hist + hist_bytes, st));
+    AsyncFree dbuf_guard{dbuf, st};
+    CUDA_OK(cudaMemcpyAsync(dbuf, h, o_hist, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaEventRecord(ev, st));
+    ClDev a{reinterpret_cast<const ifb::ClJob*>(dbuf), reinterpret_cast<const uint32_t*>(dbuf + o_first), (uint32_t)wk.jobs.size(),
+            reinterpret_cast<const ifb::ClSeg*>(dbuf + o_segs), dbuf + o_tab, reinterpret_cast<const float*>(dbuf + o_mat),
+            reinterpret_cast<unsigned long long*>(dbuf + o_hist)};
+    if (!wk.wb_jobs.empty()) {
+        ClDev w = a;
+        w.jobs = reinterpret_cast<const ifb::ClJob*>(dbuf + o_wb); w.first = reinterpret_cast<const uint32_t*>(dbuf + o_wbf);
+        w.n = (uint32_t)wk.wb_jobs.size();
+        CUDA_OK(cudaMemsetAsync(w.hist, 0, hist_bytes, st));
+        color_hist_kernel<<<(unsigned)wk.wb_ctas(), ifb::kClThreads, 0, st>>>(w);
+        CUDA_OK(cudaGetLastError());
+        color_maps_kernel<<<w.n, 256, 0, st>>>(w);
+        CUDA_OK(cudaGetLastError());
+        b->launches += 2;
+    }
+    color_apply_kernel<<<(unsigned)wk.ctas(), ifb::kClThreads, 0, st>>>(a);
+    CUDA_OK(cudaGetLastError());
+    b->launches++;
+}
+
 // Pageable host bitmaps (imageflow's Bitmap buffers are plain Vecs, aligned_buffer.rs:40-43): cudaMemcpy2DAsync from pageable memory
 // is staged by the driver on the calling thread (about 10 GB/s, and it does not overlap).  The drop-in path therefore stages such
 // bitmaps itself: the rows are copied into a pinned buffer of the pipeline slot by a few host threads in parallel, the pinned buffer
@@ -1681,6 +1735,14 @@ int ifb200_batch_orient(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, 
         if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
         std::lock_guard<std::mutex> lk(b->mu);
         orient_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
+    });
+}
+
+int ifb200_batch_color_chain(ifb200_batch* b, const ifb200_color_desc* d, size_t n, void* stream, char* err, size_t cap) {
+    return guarded(err, cap, [&] {
+        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
+        std::lock_guard<std::mutex> lk(b->mu);
+        color_chain_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
     });
 }
 

@@ -21,6 +21,7 @@
 #include "ifb_round_corners.h"     // RcJob / RcTile: planned on the host, read by round_corners_kernel
 #include "ifb_canvas.h"            // CvItem / CvTile: planned on the host, read by canvas_kernel
 #include "ifb_orient.h"            // OrItem: planned on the host, read by orient_kernel
+#include "ifb_color.h"             // ClJob / ClSeg: planned on the host, read by the colour-chain kernels
 
 namespace ifbk {
 
@@ -259,6 +260,9 @@ __global__ void __launch_bounds__(256) flip_horizontal_bgra8_v4_kernel(uint8_t* 
     }
 }
 
+// ---------------------------------------------------------------- colour chains (ColorMatrixSrgb, EnableTransparency, white balance) in one pass; own file for tests/cpu_emu
+#include "ifb_color_kernel.cuh"
+
 // ---------------------------------------------------------------- white balance (SURVEY.md section 8(f), item 4, first half)
 // flow/nodes/white_balance.rs:93-121 = three passes: per-channel histograms (graphics/histogram.rs:7-20), the area-threshold
 // byte mappings (white_balance.rs:14-48, f64 arithmetic, a handful of operations), and the in-place remap (:50-67).
@@ -299,28 +303,19 @@ __global__ void __launch_bounds__(256) histogram_bgra8_kernel(const uint8_t* __r
 // white_balance.rs:14-48.  One block of 256 threads: thread c < 3 scans channel c's histogram from both ends (both scans
 // compare against low_threshold, as the reference does), then thread v writes maps[c * 256 + v] for the three channels.
 // `high - low` is a usize subtraction in the reference: it wraps when the thresholds cross (release build semantics).
+// The arithmetic is wb_area_threshold / wb_map_byte (ifb_color_kernel.cuh), shared with the colour chain's color_maps_kernel.
 __global__ void __launch_bounds__(256) white_balance_maps_kernel(const unsigned long long* __restrict__ hist, unsigned long long total_pixels,
                                                                  double low_threshold, uint8_t* __restrict__ maps) {
     __shared__ unsigned long long lo[3], hi[3];
     const int t = threadIdx.x;
     if (t < 3) {
-        const unsigned long long* hc = hist + t * 256;
-        const double pixel_count = (double)total_pixels;
-        unsigned long long low = 0, high = 255, area = 0;
-        for (int ix = 0; ix < 256; ++ix) { area += hc[ix]; if (__ddiv_rn((double)area, pixel_count) > low_threshold) { low = ix; break; } }
-        area = 0;
-        for (int ix = 255; ix >= 0; --ix) { area += hc[ix]; if (__ddiv_rn((double)area, pixel_count) > low_threshold) { high = ix; break; } }
-        lo[t] = low; hi[t] = high;
+        unsigned long long l, h;
+        wb_area_threshold(hist + t * 256, total_pixels, low_threshold, &l, &h);
+        lo[t] = l; hi[t] = h;
     }
     __syncthreads();
 #pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        const double scale = __ddiv_rn(255.0, (double)(hi[c] - lo[c]));                       // u64 wrap-around like usize
-        const unsigned long long d = (unsigned long long)t > lo[c] ? (unsigned long long)t - lo[c] : 0ull;   // saturating_sub
-        double m = round(__dmul_rn((double)d, scale));
-        m = fmax(fmin(m, 255.0), 0.0);                                                         // NaN -> 255 -> 255, as f64::min/max
-        maps[c * 256 + t] = (uint8_t)m;
-    }
+    for (int c = 0; c < 3; ++c) maps[c * 256 + t] = wb_map_byte(lo[c], hi[c], (unsigned long long)t);
 }
 // white_balance.rs:50-67: r, g, b through their byte maps, alpha untouched, in place
 template <bool V4>

@@ -21,13 +21,6 @@ void span(const uint8_t* p, uint32_t w, uint32_t h, uint32_t stride, uintptr_t* 
 
 bool transposing(int32_t o) { return o >= 5; }
 
-// 16-byte groups per row of xlim pixels starting at `row0`: with a stride that is a multiple of 16 every row starts at the phase of
-// row0; otherwise a row may start at any of the four, and (xlim + 6) / 4 covers the widest case.
-uint32_t groups_per_row(const uint8_t* row0, uint32_t stride, uint32_t xlim) {
-    const uint32_t a0 = (uint32_t)((reinterpret_cast<uintptr_t>(row0) & 15) >> 2);
-    return (stride & 15) == 0 ? (a0 + xlim + 3) / 4 : (xlim + 6) / 4;
-}
-
 void add(OrWork& wk, const OrItem& it, uint64_t ctas) {
     if (ctas == 0) return;
     if (wk.first.empty()) wk.first.push_back(0);
@@ -43,6 +36,13 @@ void add_groups(OrWork& wk, OrItem it, uint32_t y0, uint32_t rows, uint32_t xlim
 }
 
 }  // namespace
+
+// With a stride that is a multiple of 16 every row starts at the phase of row0; otherwise a row may start at any of the four, and
+// (xlim + 6) / 4 covers the widest case.
+uint32_t groups_per_row(const uint8_t* row0, uint32_t stride, uint32_t xlim) {
+    const uint32_t a0 = (uint32_t)((reinterpret_cast<uintptr_t>(row0) & 15) >> 2);
+    return (stride & 15) == 0 ? (a0 + xlim + 3) / 4 : (xlim + 6) / 4;
+}
 
 int32_t orient_flag(int32_t o) { return o >= 2 && o <= 8 ? o : 1; }
 

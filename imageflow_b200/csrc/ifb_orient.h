@@ -39,6 +39,10 @@ struct OrWork {
     uint64_t ctas() const { return first.empty() ? 0 : first.back(); }
 };
 
+// 16-byte groups per row of xlim pixels starting at `row0`, for rows `stride` bytes apart: enough to cover every row whatever its
+// 4-byte phase modulo 16 (also used by the colour planner, ifb_color.cc).
+uint32_t groups_per_row(const uint8_t* row0, uint32_t stride, uint32_t xlim);
+
 // The orientation a flag stands for: 2..8 as they are, every other value 1 (the identity).
 int32_t orient_flag(int32_t orientation);
 

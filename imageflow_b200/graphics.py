@@ -9,7 +9,7 @@ from typing import Optional, Sequence
 
 import numpy as np
 
-from ._lib import CanvasDesc, OrientDesc, ResampleDesc, RoundCornersDesc, lib
+from ._lib import CanvasDesc, ColorDesc, ColorStep, OrientDesc, ResampleDesc, RoundCornersDesc, lib
 
 
 class Filter(enum.IntEnum):
@@ -280,8 +280,10 @@ class ExpandCanvas:
 
 @dataclass
 class EnableTransparency:
-    """EnableTransparencyMutDef (flow/nodes/enable_transparency.rs:70-86): a Bgr32 window gets A = 255 and becomes Bgra32."""
-    window: BitmapWindow
+    """EnableTransparencyMutDef (flow/nodes/enable_transparency.rs:70-86): a Bgr32 window gets A = 255 and becomes Bgra32.  With a
+    window it is a canvas operation (Batch.canvas); without one, a step of a colour chain (Batch.color_chain), where it has the
+    meaning of the expand-level node: nothing on a Bgra32 window (enable_transparency.rs:27-33)."""
+    window: Optional[BitmapWindow] = None
 
 
 def _device_of(w: BitmapWindow, default: int) -> int:
@@ -397,6 +399,8 @@ def _fill_canvas_desc(d: CanvasDesc, op, device: int):
         return done
     if isinstance(op, EnableTransparency):
         w = op.window
+        if w is None:
+            raise FlowError(ErrorKind.InvalidArgument, "EnableTransparency as a canvas operation needs a window")
         if w.alpha_meaningful:                                   # enable_transparency.rs:74-78
             raise FlowError(ErrorKind.InvalidArgument, "Need Bgr32 input image to convert to bgra32")
         d.op = _NORMALIZE_ALPHA
@@ -489,6 +493,106 @@ def apply_orientation(window: BitmapWindow, flag: int, device: int = 0):
     t = _ORIENTATION.get(int(flag), _ORIENTATION[1])[0]
     w, h = (window.h, window.w) if t else (window.w, window.h)
     return window, new_canvas(w, h, _device_of(window, device), window.alpha_meaningful), int(flag)
+
+
+# ---------------------------------------------------------------- colour chains (Batch.color_chain), named after the imageflow_types nodes
+@dataclass(eq=False)
+class ColorMatrixSrgb:
+    """Node::ColorMatrixSrgb { matrix }: window_bgra32_apply_color_matrix (graphics/color_matrix.rs:5-28), matrix[k][c] = the weight of
+    input channel k (r, g, b, a, then the bias row) in output channel c."""
+    matrix: np.ndarray
+
+    def __post_init__(self):
+        self.matrix = np.array(self.matrix, np.float32).reshape(5, 5)
+
+
+@dataclass(frozen=True)
+class WhiteBalanceHistogramAreaThresholdSrgb:
+    """Node::WhiteBalanceHistogramAreaThresholdSrgb { threshold } (flow/nodes/white_balance.rs:93-121); None = 0.006."""
+    threshold: Optional[float] = None
+
+
+class ColorFilterSrgb:
+    """Node::ColorFilterSrgb(filter): each preset returns the steps the node expands into (flow/nodes/color.rs:49-80) -- one
+    ColorMatrixSrgb of color_filter_matrix(), preceded by EnableTransparency for Alpha."""
+    @staticmethod
+    def sepia(): return [ColorMatrixSrgb(color_filter_matrix(0))]
+    @staticmethod
+    def grayscale_ntsc(): return [ColorMatrixSrgb(color_filter_matrix(1))]
+    @staticmethod
+    def grayscale_flat(): return [ColorMatrixSrgb(color_filter_matrix(2))]
+    @staticmethod
+    def grayscale_bt709(): return [ColorMatrixSrgb(color_filter_matrix(3))]
+    @staticmethod
+    def grayscale_ry(): return [ColorMatrixSrgb(color_filter_matrix(4))]
+    @staticmethod
+    def invert(): return [ColorMatrixSrgb(color_filter_matrix(5))]
+    @staticmethod
+    def alpha(p: float): return [EnableTransparency(), ColorMatrixSrgb(color_filter_matrix(6, p))]
+    @staticmethod
+    def contrast(p: float): return [ColorMatrixSrgb(color_filter_matrix(7, p))]
+    @staticmethod
+    def brightness(p: float): return [ColorMatrixSrgb(color_filter_matrix(8, p))]
+    @staticmethod
+    def saturation(p: float): return [ColorMatrixSrgb(color_filter_matrix(9, p))]
+
+
+_GRAYSCALE = {"ntsc": ColorFilterSrgb.grayscale_ntsc, "true": ColorFilterSrgb.grayscale_ntsc, "y": ColorFilterSrgb.grayscale_ntsc,
+              "flat": ColorFilterSrgb.grayscale_flat, "bt709": ColorFilterSrgb.grayscale_bt709, "ry": ColorFilterSrgb.grayscale_ry}
+
+
+def riapi_color_steps(alpha=None, brightness=None, contrast=None, saturation=None, sepia=None, grayscale=None, balance_white=None) -> list:
+    """The colour steps RIAPI's layout emits (imageflow_riapi ir4/layout.rs:562-591) from the parsed values of s.alpha, s.brightness,
+    s.contrast, s.saturation, s.sepia, s.grayscale (true / ntsc / y -> Ntsc, flat, bt709, ry) and a.balancewhite (true / area -> the
+    area threshold; other algorithms emit nothing), in the reference's order."""
+    steps = []
+    for p, preset in ((alpha, ColorFilterSrgb.alpha), (brightness, ColorFilterSrgb.brightness), (contrast, ColorFilterSrgb.contrast),
+                      (saturation, ColorFilterSrgb.saturation)):
+        if p is not None:
+            steps += preset(float(p))
+    if sepia:
+        steps += ColorFilterSrgb.sepia()
+    if grayscale is not None:
+        steps += _GRAYSCALE[str(grayscale).lower()]()
+    if balance_white is True or str(balance_white).lower() in ("true", "area"):
+        steps.append(WhiteBalanceHistogramAreaThresholdSrgb())
+    return steps
+
+
+_COLOR_MATRIX, _COLOR_ENABLE_TRANSPARENCY, _COLOR_WHITE_BALANCE = range(3)          # enum ifb200_color_step_kind
+
+
+def _struct_dtype(S):
+    def fmt(t):
+        if t is C.c_void_p:
+            return np.uint64
+        if hasattr(t, "_length_"):
+            return (np.dtype(t._type_), (t._length_,))
+        return np.dtype(t)
+    return np.dtype({"names": [n for n, _ in S._fields_], "formats": [fmt(t) for _, t in S._fields_],
+                     "offsets": [getattr(S, n).offset for n, _ in S._fields_], "itemsize": C.sizeof(S)})
+
+
+_COLOR_STEP_DTYPE, _COLOR_DESC_DTYPE = _struct_dtype(ColorStep), _struct_dtype(ColorDesc)
+
+
+def _color_steps(steps):
+    """-> (packed ifb200_color_step array, the array's address, whether the chain contains EnableTransparency, whether it contains a
+    ColorMatrixSrgb); presets' lists are flattened"""
+    flat = []
+    for s in steps:
+        flat.extend(s if isinstance(s, (list, tuple)) else [s])
+    a = np.zeros(len(flat), _COLOR_STEP_DTYPE)
+    for i, s in enumerate(flat):
+        if isinstance(s, ColorMatrixSrgb):
+            a[i]["kind"] = _COLOR_MATRIX; a[i]["matrix"] = s.matrix.reshape(25)
+        elif isinstance(s, EnableTransparency) and s.window is None:
+            a[i]["kind"] = _COLOR_ENABLE_TRANSPARENCY
+        elif isinstance(s, WhiteBalanceHistogramAreaThresholdSrgb):
+            a[i]["kind"] = _COLOR_WHITE_BALANCE; a[i]["threshold"] = -1.0 if s.threshold is None else float(s.threshold)
+        else:
+            raise FlowError(ErrorKind.InvalidArgument, f"not a colour step: {s!r}")
+    return (a, a.ctypes.data, any(isinstance(s, EnableTransparency) for s in flat), any(isinstance(s, ColorMatrixSrgb) for s in flat))
 
 
 def flow_scale_spatial(samples: np.ndarray, n: int, srgb: bool = False) -> np.ndarray:
@@ -718,6 +822,39 @@ class Batch:
             out.alpha_meaningful = inp.alpha_meaningful
         self._keep.append([(j[0]._keep, o._keep) for j, o in zip(jobs, outs)])
         return outs
+
+    def color_chain(self, jobs, stream=None) -> list:
+        """Colour chains on DEVICE windows, in place, all jobs in one kernel launch (three when a job white-balances; none when no
+        job writes a pixel), asynchronous on `stream`.  jobs: iterable of (window, steps), steps a list of ColorMatrixSrgb,
+        EnableTransparency(), WhiteBalanceHistogramAreaThresholdSrgb and ColorFilterSrgb presets (see riapi_color_steps), applied in
+        order.  No two windows may share a pixel.  Returns the windows with the metadata the nodes leave behind: BlendWithSelf
+        compositing after any ColorMatrixSrgb (ColorMatrixSrgbMutDef, flow/nodes/color.rs:29) and on a Bgr32 window that met
+        EnableTransparency, which is Bgra32 from then on (enable_transparency.rs:80-82); zero-area windows too, as the nodes still run
+        there.  White balance leaves the metadata alone.  Nothing is changed when an argument is rejected."""
+        jobs = list(jobs)
+        packed = {}
+        for _, steps in jobs:                                     # a steps list shared by many jobs is packed once
+            if id(steps) not in packed:
+                packed[id(steps)] = _color_steps(steps)
+        wins = [j[0] for j in jobs]
+        if any(w.pixel_layout != "BGRA" for w in wins):
+            raise FlowError(ErrorKind.InvalidArgument, "Only BGRA supported for colour chains")
+        a = np.zeros(len(jobs), _COLOR_DESC_DTYPE)               # filled a column at a time: no per-field ctypes marshalling
+        a["px"] = [w.ptr for w in wins]; a["w"] = [w.w for w in wins]; a["h"] = [w.h for w in wins]
+        a["stride"] = [w.stride for w in wins]; a["alpha_meaningful"] = [bool(w.alpha_meaningful) for w in wins]
+        chains = [packed[id(j[1])] for j in jobs]
+        a["steps"] = [c[1] for c in chains]; a["n_steps"] = [len(c[0]) for c in chains]
+        arr = (ColorDesc * len(jobs)).from_buffer(a)
+        buf = C.create_string_buffer(512)
+        _check(lib().ifb200_batch_color_chain(self._h, arr, len(jobs), self._stream(stream), buf, 512), buf)
+        for w, (_, _, et, matrix) in zip(wins, chains):
+            if et and not w.alpha_meaningful:
+                w.alpha_meaningful = True
+                w.compose = BitmapCompositing.BlendWithSelf
+            if matrix:
+                w.compose = BitmapCompositing.BlendWithSelf
+        self._keep.append([w._keep for w in wins])
+        return wins
 
     def flip_vertical(self, bitmap: BitmapWindow, stream=None) -> None:
         """graphics/flip.rs:10-22 on a DEVICE bitmap, in place."""

@@ -216,6 +216,33 @@ typedef struct ifb200_orient_desc {
     int32_t        orientation;                           /* EXIF flag; values other than 2..8 are the identity */
 } ifb200_orient_desc;
 
+/* One colour chain: the photometric nodes of a flow graph applied in order to one BGRA8 window, in place, byte for byte as the
+ * reference runs them node by node (each node requantises to bytes, so a chain is not one matrix):
+ *   MATRIX               ColorMatrixSrgb { matrix } = window_bgra32_apply_color_matrix (graphics/color_matrix.rs:5-28): every output
+ *                        channel from the pixel's original four bytes, the sum left to right in f32 (bias m[4][c] * 255 last), then
+ *                        uchar_clamp_ff.  NaN and infinite coefficients are not errors: they compute what the reference computes.
+ *                        ColorFilterSrgb presets are matrices (ifb200_color_filter_matrix); Alpha is ENABLE_TRANSPARENCY + MATRIX.
+ *   ENABLE_TRANSPARENCY  the EnableTransparency node (flow/nodes/enable_transparency.rs:27-33): on a Bgr32 window A = 255 and the job
+ *                        is Bgra32 from then on; on Bgra32 nothing (the node deletes itself there).
+ *   WHITE_BALANCE        WhiteBalanceHistogramAreaThresholdSrgb { threshold } (flow/nodes/white_balance.rs:93-121): R, G, B histograms
+ *                        of the whole window as the chain has left it at that step, area thresholds and byte maps in f64, R, G, B
+ *                        remapped, alpha untouched.  threshold < 0 = None (0.006), NaN refused.  At most one per job.
+ * A job with no steps or no pixels is skipped unchecked.  Only pixels are written: the bitmap metadata the nodes change stays with the
+ * caller (BlendWithSelf after any MATRIX, color.rs:29; Bgra32 + BlendWithSelf after ENABLE_TRANSPARENCY on Bgr32). */
+enum ifb200_color_step_kind { IFB200_COLOR_MATRIX = 0, IFB200_COLOR_ENABLE_TRANSPARENCY = 1, IFB200_COLOR_WHITE_BALANCE = 2 };
+#define IFB200_COLOR_MAX_STEPS 16          /* steps per job; RIAPI's s.* / a.balancewhite keys make at most 8 */
+typedef struct ifb200_color_step {
+    int32_t kind;                          /* enum ifb200_color_step_kind */
+    float   matrix[25];                    /* MATRIX: row-major [5][5] exactly as color_matrix.rs reads it (m[k][c]: input k, output c) */
+    float   threshold;                     /* WHITE_BALANCE: < 0 = None (0.006); NaN refused */
+} ifb200_color_step;
+typedef struct ifb200_color_desc {
+    uint8_t* px; uint32_t w, h, stride;    /* BGRA8 window, in place; stride in bytes */
+    int32_t  alpha_meaningful;             /* the window's format going in: Bgra32 (1) or Bgr32 (0) */
+    const ifb200_color_step* steps;        /* HOST array of n_steps steps, applied in order; read before the call returns */
+    uint32_t n_steps;
+} ifb200_color_desc;
+
 /* ---- device-resident batch API (the metric path; not in the reference) -----------------------
  * descs[i].in / .canvas are DEVICE pointers on the batch's device; color_matrix stays a HOST pointer.
  * enqueue is asynchronous on `cuda_stream`, a cudaStream_t with the usual CUDA meaning (NULL = the legacy
@@ -267,6 +294,13 @@ int  ifb200_batch_canvas(ifb200_batch* b, const ifb200_canvas_desc* d, size_t n,
  * another job of the same call reads or writes (not checked).  Argument errors are reported before anything is enqueued.  There is
  * no host-buffer variant: on a host bitmap the reference's own transpose beats a trip to the GPU. */
 int  ifb200_batch_orient(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
+/* Colour chains (ifb200_color_desc) of n DEVICE windows, in place: ONE kernel launch for all jobs when no job white-balances, three
+ * (histograms, byte maps, apply) when any does, whatever the number of jobs; none when no job writes a pixel.  Each pixel is read
+ * once and written once (read twice with a white balance).  Asynchronous on `cuda_stream`.  No two windows of a call may share a
+ * pixel (not checked).  Argument errors are reported before anything is enqueued; a second WHITE_BALANCE in one job is
+ * IFB200_ERR_NOT_IMPLEMENTED.  There is no host-buffer variant: on a host bitmap one pass of the reference's own loop costs less than
+ * the trip to the GPU and back. */
+int  ifb200_batch_color_chain(ifb200_batch* b, const ifb200_color_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
 int  ifb200_batch_sync(ifb200_batch* b, char* err, size_t err_cap);
 void ifb200_batch_destroy(ifb200_batch* b);
 /* knobs / introspection (benchmarks, tests) */

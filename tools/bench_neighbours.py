@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Measurement of the SURVEY.md section 8(f) neighbours of the resample path that are built: transpose, flips, white balance, detect_content
 and rounded corners; `bench_neighbours.py canvas` measures the canvas operations alone (canvas_rows), `bench_neighbours.py orient`
-the one-gather orientation against the reference's expansion into transposes and flips (orient_rows)
+the one-gather orientation against the reference's expansion into transposes and flips (orient_rows), `bench_neighbours.py color` the
+colour chains against the reference's node-by-node expansion (color_rows)
 (the reference benchmarks transposes at 4K / 8K in benches/bench_graphics.rs:9-62).  Inputs resident in HBM, CUDA events on
 the launching stream, >= 3 warm-up calls; a set of 64 different images per size (>= 2 GB, far larger than L2) is cycled so that
 no call finds its data in cache.  One JSON line per (operation, size) with the HBM roofline of the kernel: algorithmic
@@ -372,10 +373,94 @@ def orient_rows():
     b.sync()
 
 
+def color_rows():
+    """Colour chains (Batch.color_chain) on frames resident in HBM: 64 3840x2160 frames per call (2.1 GB, cycled, far larger than L2)
+    for RIAPI chains on both sides of the planner's table-or-matrix choice, against the reference's node-by-node expansion with the
+    existing single-window calls (ColorMatrixSrgb per step, EnableTransparency through Batch.canvas, Batch.white_balance), and against
+    a torch device-to-device copy of the same algorithmic bytes: 4 read + 4 written per pixel, plus 4 read with white balance.  Both
+    the one call and the expansion are timed in five trials: the median, and the smallest and largest.  Each row checks frame 0 of the one call against the expansion, bit for bit.  Then 1024 512x384 thumbnails with row (a) in one call,
+    with the CUDA-event time and the host wall time inside the call apart."""
+    card = _card()
+    pk, src = peak()
+    b = ifb.Batch(0)
+    stream = torch.cuda.current_stream().cuda_stream
+
+    def row(name, ms, alg, **kw):
+        cm = _copy_ceiling_ms(alg)
+        print(json.dumps({"op": "color", "row": name, "ms": ms, "algorithmic_bytes": alg, "achieved_gbs": alg / ms / 1e6,
+                          "frac_of_peak": alg / ms / 1e6 / pk, "peak_gbs": pk, "peak_source": src, "torch_copy_same_bytes_ms": cm,
+                          "frac_of_torch_copy": cm / ms, **kw, **card}), flush=True)
+
+    def expansion(win, steps, am):
+        win.alpha_meaningful = am
+        for s in steps:
+            if isinstance(s, ifb.ColorMatrixSrgb):
+                b.color_matrix(win.ptr, win.w, win.h, win.stride, s.matrix, stream)
+            elif isinstance(s, ifb.EnableTransparency):
+                if not win.alpha_meaningful:
+                    b.canvas([ifb.EnableTransparency(win)], stream)
+            else:
+                b.white_balance(win, s.threshold, stream)
+
+    def one_call(wins, steps, am):
+        for w in wins:
+            w.alpha_meaningful = am
+        b.color_chain([(w, steps) for w in wins], stream)
+
+    n, w, h = 64, 3840, 2160
+    frames = (torch.randn((n, h, w, 4), device="cuda") * 40 + 128).clamp_(0, 255).to(torch.uint8)
+    wins = [ifb.BitmapWindow.from_torch(frames[i]) for i in range(n)]
+    rows = [("a_brightness_contrast_table", dict(brightness=0.1, contrast=0.2), True),
+            ("b_saturation_sepia_matrix", dict(saturation=-0.5, sepia=True), True),
+            ("c_alpha_on_bgr32", dict(alpha=0.5), False),
+            ("d_all_seven_keys", dict(alpha=0.5, brightness=0.1, contrast=0.2, saturation=-0.3, sepia=True, grayscale="true",
+                                      balance_white=True), False),
+            ("e_balancewhite", dict(balance_white=True), True)]
+    for name, keys, am in rows:
+        steps = ifb.riapi_color_steps(**keys)
+        wb = any(isinstance(s, ifb.WhiteBalanceHistogramAreaThresholdSrgb) for s in steps)
+        before = b.kernel_launches
+        one_call(wins, steps, am)
+        launches = b.kernel_launches - before
+        # five trials each: the expansion is bound by host time (each ColorMatrixSrgb call stages its matrix and allocates on the
+        # stream) and varies from trial to trial, so its spread is reported with the median
+        one = sorted(_time_ms(lambda: one_call(wins, steps, am)) for _ in range(5))
+        exp = sorted(_time_ms(lambda: [expansion(wn, steps, am) for wn in wins], reps=3) for _ in range(5))
+        ms_one, ms_exp = one[2], exp[2]
+        keep = frames[0].clone()
+        one_call(wins[:1], steps, am)
+        got = frames[0].clone()
+        frames[0].copy_(keep)
+        expansion(wins[0], steps, am)
+        ok = bool(torch.equal(got, frames[0]))
+        row(f"{name}_64x{w}x{h}_one_call", ms_one, n * w * h * (12 if wb else 8), frames=n, size=f"{w}x{h}", keys=keys,
+            steps=len(steps), launches_per_call=launches, one_call_ms_min_max=[one[0], one[-1]], expansion_ms=ms_exp,
+            expansion_ms_min_max=[exp[0], exp[-1]], one_call_vs_expansion=ms_exp / ms_one,
+            one_call_vs_expansion_range=[exp[0] / one[-1], exp[-1] / one[0]], bit_exact_vs_expansion=ok)
+    del frames, wins
+    torch.cuda.empty_cache()
+
+    n, w, h = 1024, 512, 384
+    thumbs = torch.randint(0, 256, (n, h, w, 4), dtype=torch.uint8, device="cuda")
+    twins = [ifb.BitmapWindow.from_torch(thumbs[i], alpha_meaningful=True) for i in range(n)]
+    steps = ifb.riapi_color_steps(brightness=0.1, contrast=0.2)
+    ev, host = _time_event_and_host_ms(lambda: b.color_chain([(wn, steps) for wn in twins], stream))
+    keep = thumbs[7].clone()
+    b.color_chain([(twins[7], steps)], stream)
+    got = thumbs[7].clone()
+    thumbs[7].copy_(keep)
+    expansion(twins[7], steps, True)
+    row(f"a_brightness_contrast_table_{n}x{w}x{h}_one_call", ev, n * w * h * 8, frames=n, host_wall_ms=host,
+        bit_exact_vs_expansion=bool(torch.equal(got, thumbs[7])))
+    b.sync()
+
+
 if __name__ == "__main__":
     if sys.argv[1:] == ["canvas"]:
         canvas_rows()
     elif sys.argv[1:] == ["orient"]:
         orient_rows()
+    elif sys.argv[1:] == ["color"]:
+        color_rows()
     else:
         main()
