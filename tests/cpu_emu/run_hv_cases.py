@@ -6,6 +6,7 @@ import numpy as np
 
 import imageflow_b200 as ifb
 import oracle
+from imageflow_b200 import synth
 from tests import cpu_emu, util
 
 # (in_w, in_h, out_w, out_h, filter, kwargs of run_hv)
@@ -23,6 +24,15 @@ CASES = [
     (1024, 64, 96, 17, 13, dict(alpha=True, sharpen=50.0)),                  # CatmullRom, sharpen
     (128, 128, 37, 41, 24, dict()),                                          # Box
     (400, 300, 100, 75, 4, dict(alpha=True, linear=False, strip_cols=16)),   # Ginseng (ring depth 6), sRGB space
+    # cut-out content (synth.cutout_np over synth.cutout_canvas_np): alpha exactly 0, negative, tiny, above 1 and next to 0.994
+    # before the store, fa == 0 and fa < 0 in BlendWithSelf (tests/test_alpha_edges_oracle.py checks that these are reached)
+    (640, 480, 200, 150, 2, dict(content="cutout", alpha=True)),
+    (640, 480, 200, 150, 2, dict(content="cutout", alpha=True, compose=1)),
+    (640, 480, 200, 150, 2, dict(content="cutout", alpha=True, compose=2, linear=False, cm="sepia")),
+    (960, 540, 128, 128, 6, dict(content="cutout", alpha=True, compose=1, linear=False)),       # Lanczos3: ring depth 6
+    (960, 540, 128, 128, 6, dict(content="cutout", alpha=True, compose=2)),
+    (512, 384, 128, 96, 2, dict(content="cutout", alpha=True, compose=1, cm="sepia", n_bands=2)),
+    (512, 384, 128, 96, 2, dict(content="cutout", alpha=False, compose=1, linear=False)),
 ]
 
 
@@ -36,8 +46,11 @@ def run(so, limit=None):
         cm = ifb.color_filter_matrix(0) if cm == "sepia" else None
         common = dict(filter=flt, alpha_meaningful=alpha, linear=kw.pop("linear", True), compose=kw.pop("compose", 0), matte=(40, 120, 250, 200),
                       color_matrix=cm, sharpen=kw.pop("sharpen", 0.0))
-        inp = util.noise(iw, ih, seed=iw + oh, alpha_mode="mixed" if alpha else "opaque")
-        canvas = util.noise(ow + 5, oh + 3, seed=3, alpha_mode="mixed")
+        if kw.pop("content", "noise") == "cutout":
+            inp, canvas = synth.cutout_np(iw, ih, seed=iw + oh), synth.cutout_canvas_np(ow + 5, oh + 3, seed=3)
+        else:
+            inp = util.noise(iw, ih, seed=iw + oh, alpha_mode="mixed" if alpha else "opaque")
+            canvas = util.noise(ow + 5, oh + 3, seed=3, alpha_mode="mixed")
         exp = canvas.copy()
         oracle.scale_and_render(inp, exp, x=2, y=1, w=ow, h=oh, **common)
         outs = cpu_emu.run_hv(L, ifb, inp, canvas, x=2, y=1, w=ow, h=oh, **common, **kw)

@@ -20,7 +20,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def test_emulated_hv_kernel_is_bit_exact(tmp_path):
     so = cpu_emu.build_hv(str(tmp_path))
-    assert run_hv_cases.run(so) >= 13
+    assert run_hv_cases.run(so) >= 20
 
 
 def test_emulated_hv_kernel_under_address_sanitizer(tmp_path):
