@@ -16,6 +16,8 @@ Host-side mirror of the reference seam (paths relative to the imageflow checkout
       orientation_of; RIAPI's add_rotate / add_flip as riapi_rotate_steps / riapi_flip_steps)
   flow/nodes/color.rs, enable_transparency.rs, white_balance.rs  ColorMatrixSrgb, ColorFilterSrgb presets, EnableTransparency and
       WhiteBalanceHistogramAreaThresholdSrgb as one chain per frame (Batch.color_chain; RIAPI's s.* / a.balancewhite as riapi_color_steps)
+  flow/nodes/watermark.rs, imageflow_riapi ir4/layout.rs + sizing.rs  Watermark: its layout (watermark_layout, process_constraint) and
+      every frame's composite from one resample per distinct watermark (Batch.watermark; RIAPI's placement as riapi_watermark_placement)
   c_components/lib/codecs_jpeg_idct_fast.c  flow_scale_spatial[_srgb]_NxN (decode-time JPEG block scalers)
 All arithmetic runs in hand-written sm_90a kernels inside libifb200.so (include/ifb200.h);
 this package only marshals arguments.  Nothing here imports the CPU oracle.
@@ -28,7 +30,8 @@ from .graphics import (Batch, apply_matte, BitmapCompositing, BitmapWindow, Erro
                        FillRect, CopyRectToCanvas, ExpandCanvas, EnableTransparency, new_canvas, watermark_red_dot, region, region_percent,
                        ApplyOrientation, Rotate90, Rotate180, Rotate270, FlipH, FlipV, Transpose, orientation_of, riapi_rotate_steps,
                        riapi_flip_steps, apply_orientation, ColorMatrixSrgb, ColorFilterSrgb, WhiteBalanceHistogramAreaThresholdSrgb,
-                       riapi_color_steps)
+                       riapi_color_steps, Watermark, WatermarkConstraintBox, WatermarkConstraintMode, ConstraintGravity, WatermarkDraw,
+                       process_constraint, watermark_layout, riapi_watermark_placement)
 from ._lib import LIB_PATH, ResampleDesc, lib
 
 __all__ = [
@@ -40,5 +43,6 @@ __all__ = [
     "FillRect", "CopyRectToCanvas", "ExpandCanvas", "EnableTransparency", "new_canvas", "watermark_red_dot", "region", "region_percent",
     "ApplyOrientation", "Rotate90", "Rotate180", "Rotate270", "FlipH", "FlipV", "Transpose", "orientation_of", "riapi_rotate_steps",
     "riapi_flip_steps", "apply_orientation", "ColorMatrixSrgb", "ColorFilterSrgb", "WhiteBalanceHistogramAreaThresholdSrgb",
-    "riapi_color_steps", "LIB_PATH", "ResampleDesc", "lib",
+    "riapi_color_steps", "Watermark", "WatermarkConstraintBox", "WatermarkConstraintMode", "ConstraintGravity", "WatermarkDraw",
+    "process_constraint", "watermark_layout", "riapi_watermark_placement", "LIB_PATH", "ResampleDesc", "lib",
 ]

@@ -21,7 +21,7 @@ SYMBOLS = [
     "ifb200_batch_destroy", "ifb200_batch_set_option", "ifb200_batch_kernel_launches", "ifb200_batch_host_profile",
     "ifb200_batch_fused_jobs", "ifb200_batch_generic_jobs", "ifb200_batch_tile_jobs", "ifb200_batch_ring_status", "ifb200_hv_plan_tables",
     "ifb200_block_scale_u8", "ifb200_batch_block_scale", "ifb200_round_corners_bgra8", "ifb200_batch_round_corners",
-    "ifb200_batch_canvas", "ifb200_batch_orient", "ifb200_batch_color_chain",
+    "ifb200_batch_canvas", "ifb200_batch_orient", "ifb200_batch_color_chain", "ifb200_batch_watermark",
 ]
 
 
@@ -75,6 +75,11 @@ class ColorDesc(C.Structure):
         ("px", C.c_void_p), ("w", C.c_uint32), ("h", C.c_uint32), ("stride", C.c_uint32), ("alpha_meaningful", C.c_int32),
         ("steps", C.c_void_p), ("n_steps", C.c_uint32),
     ]
+
+
+class WatermarkDesc(C.Structure):
+    """struct ifb200_watermark_desc"""
+    _fields_ = [("draw", ResampleDesc), ("opacity", C.c_float)]
 
 
 _lib = None
@@ -169,6 +174,8 @@ def lib() -> C.CDLL:
     L.ifb200_batch_orient.restype = C.c_int
     L.ifb200_batch_color_chain.argtypes = [C.c_void_p, C.POINTER(ColorDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_color_chain.restype = C.c_int
+    L.ifb200_batch_watermark.argtypes = [C.c_void_p, C.POINTER(WatermarkDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
+    L.ifb200_batch_watermark.restype = C.c_int
     L.ifb200_batch_ring_status.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_ring_status.restype = C.c_int
     _lib = L

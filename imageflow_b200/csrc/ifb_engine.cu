@@ -702,14 +702,9 @@ void ensure_axes(ifb200_batch* b, cudaStream_t st, Plan& p) {
 }
 
 void validate(const ifb200_resample_desc& d) {
-    if (!d.in || !d.canvas) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null bitmap pointer");
-    if ((uint64_t)d.h + d.y > d.cv_h || (uint64_t)d.w + d.x > d.cv_w)                     // scaling.rs:24-29
-        IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "Destination rectangle for scale2d is out of bounds");
-    if (d.w == 0 || d.h == 0 || d.in_w == 0 || d.in_h == 0) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "empty bitmap");
-    if (d.in_stride < d.in_w * 4ull || d.cv_stride < d.cv_w * 4ull || (d.in_stride & 3) || (d.cv_stride & 3))
-        IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "stride smaller than a BGRA row or not a multiple of 4");
-    if (d.compose < 0 || d.compose > 2) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "unknown compositing mode %d", d.compose);
-    if (d.filter < 1 || d.filter > 31) IFB_THROW(IFB200_ERR_BAD_FILTER, "unknown filter id %d", d.filter);
+    int code = 0;
+    const std::string why = ifb::resample_check(d, &code);                // ifb_watermark.cc: shared with ifb200_batch_watermark
+    if (!why.empty()) IFB_THROW(code, "%s", why.c_str());
 }
 
 JobDev make_job(const ifb200_resample_desc& d, const float* t_lin_host, const float* t_srgb_host) {
@@ -1343,6 +1338,138 @@ void color_chain_locked(ifb200_batch* b, const ifb200_color_desc* d, size_t n, c
     b->launches++;
 }
 
+// The watermarks of ifb200_batch_watermark (ifb_watermark.h): every descriptor is checked and every plan built before anything is
+// enqueued.  The groups are then cut into chunks of consecutive groups whose F and private copies fit in kWmScratchBytes (one chunk for
+// any call whose distinct watermarks need less; a larger group is a chunk alone), and each chunk, on `st`, in turn reuses one pooled
+// scratch buffer: its groups with an opacity get a private copy of their window and ONE colour-chain launch over the copies
+// (EnableTransparency + the Alpha matrix); each distinct geometry gets the generic H pass and vpass_f_kernel over all its groups; and ONE
+// composite launch writes every job of the chunk.  The upload is the groups, the jobs and one JobDev per group, O(jobs + groups).
+constexpr size_t kWmScratchBytes = (size_t)1 << 30;
+
+void watermark_locked(ifb200_batch* b, const ifb200_watermark_desc* d, size_t n, cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    Tick tk_all(b->prof.enqueue);
+    for (size_t i = 0; i < n; ++i) {
+        int code = 0;
+        const std::string why = ifb::watermark_check(d[i], &code);
+        if (!why.empty()) IFB_THROW(code, "watermark job %zu: %s", i, why.c_str());
+    }
+    host_tables();
+    ifb::WmWork wk;
+    ifb::watermark_plan(d, n, g_t_lin_host, g_t_srgb_host, wk);
+    if (wk.groups.empty()) return;
+    if (wk.ctas() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
+    DeviceScope dev_scope_(b->device);
+    const uint32_t ng = (uint32_t)wk.groups.size();
+    std::vector<ifb200_resample_desc> reps(ng);
+    for (uint32_t g = 0; g < ng; ++g) reps[g] = d[wk.rep[g]].draw;
+    { Tick tk(b->prof.plans); b->prebuild_plans(reps.data(), ng); }
+    std::vector<Plan*> plan(ng);
+    for (uint32_t g = 0; g < ng; ++g) { Tick tk(b->prof.plans); plan[g] = &b->plan_for(reps[g]); }      // may throw: nothing enqueued yet
+    auto at = [](size_t x) { return (x + 255) / 256 * 256; };
+    auto f_size = [&](uint32_t g) { return (size_t)wk.groups[g].w * wk.groups[g].h * 16u; };
+    auto copy_size = [&](uint32_t g) { return wk.opacity[g] < 1.0f ? at((size_t)reps[g].in_w * reps[g].in_h * 4u) : (size_t)0; };
+    // chunks; inside a chunk, the groups by geometry in first-seen order, their F consecutive (vpass_f_kernel's blockIdx.z), then the copies
+    struct Chunk { uint32_t g0, g1; std::vector<std::pair<Plan*, std::vector<uint32_t>>> geo; };
+    std::vector<Chunk> chunks;
+    std::vector<size_t> f_off(ng), copy_off(ng, SIZE_MAX);
+    size_t scratch_bytes = 0;
+    for (uint32_t g = 0; g < ng;) {
+        Chunk c{g, g, {}};
+        for (size_t bytes = 0; g < ng && (g == c.g0 || bytes + f_size(g) + copy_size(g) <= kWmScratchBytes); ++g) bytes += f_size(g) + copy_size(g);
+        c.g1 = g;
+        for (uint32_t k = c.g0; k < c.g1; ++k) {
+            auto it = std::find_if(c.geo.begin(), c.geo.end(), [&](const auto& e) { return e.first == plan[k]; });
+            if (it == c.geo.end()) { c.geo.push_back({plan[k], {}}); it = c.geo.end() - 1; }
+            it->second.push_back(k);
+        }
+        size_t off = 0;
+        for (auto& e : c.geo)
+            for (uint32_t k : e.second) { f_off[k] = off; off += f_size(k); }
+        for (uint32_t k = c.g0; k < c.g1; ++k)
+            if (copy_size(k)) { copy_off[k] = off; off += copy_size(k); }
+        scratch_bytes = std::max(scratch_bytes, off);
+        chunks.push_back(std::move(c));
+    }
+    uint8_t* scratch = nullptr;
+    CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&scratch), scratch_bytes, st));
+    AsyncFree scratch_guard{scratch, st};
+    // the H pass jobs: one per group, reading the caller's window or its private copy
+    std::vector<JobDev> hjobs(ng);
+    std::vector<uint32_t> hpos(ng);
+    {
+        uint32_t k = 0;
+        for (auto& c : chunks)
+            for (auto& e : c.geo)
+                for (uint32_t g : e.second) {
+                    ifb200_resample_desc r = reps[g];
+                    if (copy_off[g] != SIZE_MAX) { r.in = scratch + copy_off[g]; r.in_stride = r.in_w * 4u; r.alpha_meaningful = 1; }
+                    r.compose = IFB200_REPLACE_SELF; r.color_matrix = nullptr;
+                    hjobs[k] = make_job(r, g_t_lin_host, g_t_srgb_host);
+                    hpos[g] = k++;
+                }
+    }
+    for (uint32_t g = 0; g < ng; ++g) wk.groups[g].f = reinterpret_cast<const float*>(scratch + f_off[g]);
+    // the plan goes up in one copy
+    const size_t o_jobs = at(ng * sizeof(ifb::WmGroup)), o_h = o_jobs + at(wk.jobs.size() * sizeof(ifb::WmJob)), total = o_h + ng * sizeof(JobDev);
+    cudaEvent_t ev;
+    uint8_t* h = static_cast<uint8_t*>(b->stage(total, &ev));
+    memcpy(h, wk.groups.data(), ng * sizeof(ifb::WmGroup));
+    memcpy(h + o_jobs, wk.jobs.data(), wk.jobs.size() * sizeof(ifb::WmJob));
+    memcpy(h + o_h, hjobs.data(), ng * sizeof(JobDev));
+    uint8_t* dbuf = nullptr;
+    CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&dbuf), total, st));
+    AsyncFree dbuf_guard{dbuf, st};
+    CUDA_OK(cudaMemcpyAsync(dbuf, h, total, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaEventRecord(ev, st));
+    std::vector<ifb200_color_step> steps(2 * ng);
+    for (const Chunk& c : chunks) {
+        // 1. opacity: private copies, then the existing colour chain on them (one launch)
+        std::vector<ifb200_color_desc> cds;
+        for (uint32_t g = c.g0; g < c.g1; ++g) {
+            if (copy_off[g] == SIZE_MAX) continue;
+            const ifb200_resample_desc& r = reps[g];
+            CUDA_OK(cudaMemcpy2DAsync(scratch + copy_off[g], (size_t)r.in_w * 4u, r.in, r.in_stride, (size_t)r.in_w * 4u, r.in_h, cudaMemcpyDeviceToDevice, st));
+            ifb200_color_step* s = &steps[2 * g];
+            memset(s, 0, 2 * sizeof(ifb200_color_step));
+            s[0].kind = IFB200_COLOR_ENABLE_TRANSPARENCY;
+            s[1].kind = IFB200_COLOR_MATRIX;
+            ifb::color_filter_matrix(6, wk.opacity[g], s[1].matrix);            // ColorFilterSrgb::Alpha (flow/nodes/color.rs)
+            cds.push_back(ifb200_color_desc{scratch + copy_off[g], r.in_w, r.in_h, r.in_w * 4u, r.alpha_meaningful ? 1 : 0, s, 2u});
+        }
+        if (!cds.empty()) color_chain_locked(b, cds.data(), cds.size(), st);
+        // 2. F of every group: the generic H pass + vpass_f_kernel, per geometry, in chunks of at most ~1 GiB of intermediate
+        for (auto& e : c.geo) {
+            Plan& p = *e.first;
+            ensure_axes(b, st, p);
+            const uint32_t g0 = e.second.front();
+            const size_t nj = e.second.size(), per = (size_t)p.in_h * p.out_w * sizeof(float4);
+            const size_t chunk = std::max<size_t>(1, std::min<size_t>(std::min<size_t>(nj, 65535), ((size_t)1 << 30) / std::max<size_t>(per, 1)));
+            float4* inter = nullptr;
+            CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&inter), per * chunk, st));
+            AsyncFree inter_guard{inter, st};
+            const JobDev* hj = reinterpret_cast<const JobDev*>(dbuf + o_h) + hpos[g0];
+            float4* fg = reinterpret_cast<float4*>(scratch + f_off[g0]);
+            for (size_t off = 0; off < nj; off += chunk) {
+                const size_t cnt = std::min(chunk, nj - off);
+                dim3 gh((p.out_w + 127) / 128, std::min<uint32_t>(p.in_h, 65535u), (unsigned)cnt);
+                hpass_generic_kernel<<<gh, 128, 0, st>>>(hj + off, b->tables, p.dh.view(*p.axes), p.in_h, p.out_w, inter);
+                CUDA_OK(cudaGetLastError());
+                dim3 gv((p.out_w + 127) / 128, std::min<uint32_t>(p.out_h, 65535u), (unsigned)cnt);
+                vpass_f_kernel<<<gv, 128, 0, st>>>(p.dv.view(*p.axes), p.in_h, p.out_w, p.out_h, inter, fg + off * p.out_h * p.out_w);
+                CUDA_OK(cudaGetLastError());
+                b->launches += 2;
+            }
+        }
+        // 3. every composite of the chunk in one launch
+        const uint32_t cta0 = wk.groups[c.g0].first, cta1 = c.g1 < ng ? wk.groups[c.g1].first : (uint32_t)wk.ctas();
+        watermark_composite_kernel<<<cta1 - cta0, ifb::kWmThreads, 0, st>>>(reinterpret_cast<const ifb::WmGroup*>(dbuf) + c.g0, c.g1 - c.g0,
+                                                                            reinterpret_cast<const ifb::WmJob*>(dbuf + o_jobs), b->tables, cta0);
+        CUDA_OK(cudaGetLastError());
+        b->launches++;
+    }
+}
+
 // Pageable host bitmaps (imageflow's Bitmap buffers are plain Vecs, aligned_buffer.rs:40-43): cudaMemcpy2DAsync from pageable memory
 // is staged by the driver on the calling thread (about 10 GB/s, and it does not overlap).  The drop-in path therefore stages such
 // bitmaps itself: the rows are copied into a pinned buffer of the pipeline slot by a few host threads in parallel, the pinned buffer
@@ -1743,6 +1870,14 @@ int ifb200_batch_color_chain(ifb200_batch* b, const ifb200_color_desc* d, size_t
         if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
         std::lock_guard<std::mutex> lk(b->mu);
         color_chain_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
+    });
+}
+
+int ifb200_batch_watermark(ifb200_batch* b, const ifb200_watermark_desc* d, size_t n, void* stream, char* err, size_t cap) {
+    return guarded(err, cap, [&] {
+        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
+        std::lock_guard<std::mutex> lk(b->mu);
+        watermark_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
     });
 }
 

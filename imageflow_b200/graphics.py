@@ -9,7 +9,7 @@ from typing import Optional, Sequence
 
 import numpy as np
 
-from ._lib import CanvasDesc, ColorDesc, ColorStep, OrientDesc, ResampleDesc, RoundCornersDesc, lib
+from ._lib import CanvasDesc, ColorDesc, ColorStep, OrientDesc, ResampleDesc, RoundCornersDesc, WatermarkDesc, lib
 
 
 class Filter(enum.IntEnum):
@@ -39,6 +39,7 @@ class ErrorKind(enum.IntEnum):
     Ok = 0; InvalidArgument = 1; MethodNotImplemented = 2; InvalidState = 3
     TotalWeightZero = 10; SourcePixelCountTooLarge = 11; NoPixelInputs = 12; BadFilter = 13; Capacity = 14
     NoDevice = 20; CudaError = 21; OutOfMemory = 22
+    InvalidNodeParams = 100          # raised by the mirror's node layouts (watermark_layout), never returned by the library
 
 
 class FlowError(RuntimeError):
@@ -595,6 +596,303 @@ def _color_steps(steps):
     return (a, a.ctypes.data, any(isinstance(s, EnableTransparency) for s in flat), any(isinstance(s, ColorMatrixSrgb) for s in flat))
 
 
+# ---------------------------------------------------------------- watermarks (Batch.watermark), named after the imageflow_types records
+class WatermarkConstraintMode(enum.Enum):
+    """imageflow_types WatermarkConstraintMode (lib.rs:1022-1041); each maps onto the ConstraintMode of the same name."""
+    Distort = "distort"; Within = "within"; Fit = "fit"; WithinCrop = "within_crop"; FitCrop = "fit_crop"
+
+
+@dataclass(frozen=True)
+class ConstraintGravity:
+    """imageflow_types ConstraintGravity: Center (x = y = None) or Percentage { x, y } (f32 percentages)."""
+    x: Optional[float] = None
+    y: Optional[float] = None
+
+    @classmethod
+    def center(cls) -> "ConstraintGravity":
+        return cls()
+
+    @classmethod
+    def percentage(cls, x: float, y: float) -> "ConstraintGravity":
+        return cls(float(x), float(y))
+
+
+@dataclass(frozen=True)
+class WatermarkConstraintBox:
+    """imageflow_types WatermarkConstraintBox (lib.rs:1078-1087): ImagePercentage / CanvasPercentage { x1, y1, x2, y2 } (f32) and
+    ImageMargins / CanvasMargins { left, top, right, bottom } (u32), `values` in field order."""
+    kind: str
+    values: tuple
+    IMAGE_PERCENTAGE, IMAGE_MARGINS, CANVAS_PERCENTAGE, CANVAS_MARGINS = "image_percentage", "image_margins", "canvas_percentage", "canvas_margins"
+
+    @classmethod
+    def image_percentage(cls, x1, y1, x2, y2): return cls(cls.IMAGE_PERCENTAGE, tuple(float(v) for v in (x1, y1, x2, y2)))
+    @classmethod
+    def canvas_percentage(cls, x1, y1, x2, y2): return cls(cls.CANVAS_PERCENTAGE, tuple(float(v) for v in (x1, y1, x2, y2)))
+    @classmethod
+    def image_margins(cls, left, top, right, bottom): return cls(cls.IMAGE_MARGINS, tuple(int(v) for v in (left, top, right, bottom)))
+    @classmethod
+    def canvas_margins(cls, left, top, right, bottom): return cls(cls.CANVAS_MARGINS, tuple(int(v) for v in (left, top, right, bottom)))
+
+
+@dataclass(frozen=True)
+class Watermark:
+    """imageflow_types Watermark (lib.rs:1092-1101).  `hints` is accepted and, as in the reference, not used: the expansion's
+    DrawImageExact gets `constraint.hints`, which is None (flow/nodes/watermark.rs:121,180)."""
+    io_id: int = 0
+    fit_box: Optional[WatermarkConstraintBox] = None
+    fit_mode: Optional[WatermarkConstraintMode] = None
+    gravity: Optional[ConstraintGravity] = None
+    min_canvas_width: Optional[int] = None
+    min_canvas_height: Optional[int] = None
+    opacity: Optional[float] = None
+    hints: object = None
+
+
+@dataclass(frozen=True)
+class WatermarkDraw:
+    """What WatermarkDef::expand emits for one frame: Crop { crop } of the watermark (None: no crop), ColorFilterSrgb::Alpha(opacity)
+    (None: no opacity step) and DrawImageExact { x, y, w, h } with the filter scale_render.rs:251-259 picks for hints None; no sharpen,
+    linear light."""
+    crop: Optional[tuple]
+    x: int
+    y: int
+    w: int
+    h: int
+    filter: Filter
+    opacity: Optional[float]
+
+
+_F32 = np.float32
+_I32_MAX = 2 ** 31 - 1
+
+
+def _round_f64(v: float) -> float:
+    """f64::round: half away from zero (exact: x - trunc(x) has no rounding error)"""
+    import math
+    if not math.isfinite(v):
+        return v
+    t = float(math.trunc(v))
+    if abs(v - t) >= 0.5:
+        t += math.copysign(1.0, v)
+    return t
+
+
+def _clamp_f32(v, lo: float, hi: float):
+    """f32::clamp: NaN stays NaN"""
+    v = _F32(v)
+    return v if v != v else _F32(min(max(v, _F32(lo)), _F32(hi)))
+
+
+class _LayoutError(Exception):
+    pass
+
+
+class _Ratio:
+    """sizing.rs AspectRatio: a size and the ratio it stands for"""
+    __slots__ = ("w", "h")
+
+    def __init__(self, w: int, h: int):
+        if w < 1 or h < 1:
+            raise _LayoutError(f"InvalidDimensions {w}x{h}")
+        self.w, self.h = int(w), int(h)
+
+    def ratio(self) -> float:
+        return float(self.w) / float(self.h)
+
+    def aspect_wider_than(self, o: "_Ratio") -> bool:
+        return o.ratio() > self.ratio()
+
+    def loss_w(self, tw: int) -> float:
+        rounded_y = _round_f64(float(self.h) * (float(tw) / float(self.w)))
+        return abs(float(tw) - rounded_y * self.ratio())
+
+    def loss_h(self, th: int) -> float:
+        rounded_x = _round_f64(float(self.w) * (float(th) / float(self.h)))
+        return abs(float(th) - rounded_x / self.ratio())
+
+    def proportional(self, basis: int, basis_is_width: bool, target: Optional["_Ratio"]) -> int:
+        """sizing.rs:118-184, f64 throughout"""
+        import sys
+        snap = 1.0 - sys.float_info.epsilon
+        if target is not None:
+            snap = self.loss_h(target.h) if basis_is_width else self.loss_w(target.w)
+        ratio = self.ratio()
+        snap_a = self.h if basis_is_width else self.w
+        snap_b = (target.h if basis_is_width else target.w) if target is not None else snap_a
+        fl = float(basis) / ratio if basis_is_width else ratio * float(basis)
+        da, db = fl - float(snap_a), fl - float(snap_b)
+        if abs(da) <= snap and abs(da) <= abs(db):
+            v = snap_a
+        elif abs(db) <= snap:
+            v = snap_b
+        else:
+            r = _round_f64(fl)
+            if r <= -2.0 ** 31 or r >= float(_I32_MAX):
+                raise _LayoutError("ValueScalingFailed")
+            v = int(r)
+        if v < 0:
+            raise _LayoutError("ValueScalingFailed")
+        return 1 if v == 0 else v
+
+    def box_of(self, target: "_Ratio", inner: bool) -> "_Ratio":
+        if target.aspect_wider_than(self) == inner:
+            return _Ratio(target.w, self.proportional(target.w, True, target))
+        return _Ratio(self.proportional(target.h, False, target), target.h)
+
+    def intersection(self, o: "_Ratio") -> "_Ratio":
+        return _Ratio(min(self.w, o.w), min(self.h, o.h))
+
+    def distort_with(self, old: "_Ratio", new: "_Ratio") -> "_Ratio":
+        def mult(v, num, den):                                 # i64 multiply and truncating divide, then `as i32`
+            q = abs(v * num) // abs(den) * (1 if (v * num >= 0) == (den > 0) else -1)
+            return (q + 2 ** 31) % 2 ** 32 - 2 ** 31
+        return _Ratio(mult(self.w, new.w, old.w), mult(self.h, new.h, old.h))
+
+
+def _cmp(a: int, b: int) -> int:
+    return (a > b) - (a < b)
+
+
+# The sizing steps of the five watermark modes (Ir4Layout::get_instructions + build_constraints, layout.rs:162-332): (FitMode, ScaleMode)
+# = Distort (Stretch, Both), Within (Max, DownscaleOnly), Fit (Max, Both), WithinCrop (Crop, DownscaleOnly), FitCrop (Crop, Both).
+# Conditions compare the canvas with the target (sizing.rs:433-435): ("either", 1) = Cond::Either(Greater), ("either", -1) = Either(Less),
+# ("l1s1",) = Larger1DSmaller1D.
+_MODE_STEPS = {
+    WatermarkConstraintMode.Distort: [("distort",)],
+    WatermarkConstraintMode.Within: [("skip_unless", ("either", 1)), ("scale_inner",)],
+    WatermarkConstraintMode.Fit: [("scale_inner",)],
+    WatermarkConstraintMode.WithinCrop: [("skip_if", ("either", -1)), ("scale_outer",), ("crop",), ("begin",), ("skip_unless", ("l1s1",)),
+                                         ("crop_intersection",)],
+    WatermarkConstraintMode.FitCrop: [("scale_outer",), ("crop",)],
+}
+
+
+def _ir4_gravity1d(p, inner: int, outer: int) -> int:
+    """Ir4Layout::gravity1d (layout.rs:673-683): f32, clamped to [0, outer - inner]"""
+    if (outer < inner and inner < 1) or outer < 1:
+        raise _LayoutError("align")
+    ratio = _clamp_f32(p, 0.0, 100.0) / _F32(100)
+    return max(0, min(_round_f32(_F32(outer - inner) * ratio), outer - inner))
+
+
+def _gravity_xy(gravity: Optional[ConstraintGravity]):
+    return (50.0, 50.0) if gravity is None or gravity.x is None else (gravity.x, gravity.y)
+
+
+def process_constraint(src_w: int, src_h: int, mode: WatermarkConstraintMode, w: int, h: int, gravity: Optional[ConstraintGravity] = None):
+    """Ir4Layout::process_constraint (imageflow_riapi ir4/layout.rs:334-412) for the modes a watermark can ask for, with both w and h
+    given: -> (crop [x1, y1, x2, y2] of the source or None, scale_to (w, h)).  The reference panics (unwrap) on a layout error; here it
+    is FlowError(InvalidState)."""
+    try:
+        initial = _Ratio(src_w, src_h)
+        target = _Ratio(w, h)                                  # get_ideal_target_size with w, h >= 1 and zoom 1 (layout.rs:93-131)
+        lay = {"source": initial, "target": target, "canvas": initial, "image": initial}
+
+        def crop_to(t: _Ratio):
+            if t.w > lay["canvas"].w or t.h > lay["canvas"].h:
+                raise _LayoutError("ImpossibleCrop")
+            img = lay["image"].intersection(t)
+            lay.update(source=img.box_of(lay["source"], True), image=img, canvas=t)
+
+        def cond(c) -> bool:
+            cw, ch = _cmp(lay["canvas"].w, target.w), _cmp(lay["canvas"].h, target.h)
+            return (cw == c[1] or ch == c[1]) if c[0] == "either" else (cw, ch) in ((1, -1), (-1, 1))
+
+        skipping = False
+        for st in _MODE_STEPS[WatermarkConstraintMode(mode)]:
+            if st[0] == "skip_if" and cond(st[1]) or st[0] == "skip_unless" and not cond(st[1]):
+                skipping = True
+            elif st[0] == "begin":
+                skipping = False
+            if skipping or st[0] in ("skip_if", "skip_unless", "begin"):
+                continue
+            if st[0] in ("scale_inner", "scale_outer"):
+                cv = lay["canvas"].box_of(target, st[0] == "scale_inner")
+                lay.update(image=lay["image"].distort_with(lay["canvas"], cv), canvas=cv)
+            elif st[0] == "distort":
+                lay.update(image=lay["image"].distort_with(lay["canvas"], target), canvas=target)
+            elif st[0] == "crop":
+                crop_to(target)
+            else:                                              # crop_intersection
+                crop_to(lay["image"].intersection(target))
+        new_crop = lay["source"]
+        gx, gy = _gravity_xy(gravity)
+        cx, cy = _ir4_gravity1d(gx, new_crop.w, initial.w), _ir4_gravity1d(gy, new_crop.h, initial.h)
+    except _LayoutError as e:
+        raise FlowError(ErrorKind.InvalidState, f"watermark layout failed: {e}") from None
+    crop = None
+    if cx > 0 or cy > 0 or (new_crop.w, new_crop.h) != (initial.w, initial.h):
+        crop = [cx, cy, cx + new_crop.w, cy + new_crop.h]
+    return crop, (lay["image"].w, lay["image"].h)
+
+
+def _i32(v: int) -> int:
+    return (int(v) + 2 ** 31) % 2 ** 32 - 2 ** 31
+
+
+def _fit_box(w: int, h: int, fit_box: Optional[WatermarkConstraintBox]):
+    """WatermarkDef::get_bounding_box (watermark.rs:11-58): (x1, y1, x2, y2), or None when the box is not at least 1x1"""
+    if fit_box is None:
+        return 0, 0, w, h
+    if fit_box.kind in (WatermarkConstraintBox.IMAGE_MARGINS, WatermarkConstraintBox.CANVAS_MARGINS):
+        left, top, right, bottom = fit_box.values
+        if (left + right) % 2 ** 32 < w and (top + bottom) % 2 ** 32 < h:          # u32 addition
+            return _i32(left), _i32(top), w - _i32(right), h - _i32(bottom)
+        return None
+
+    def px(p, c):
+        return _round_f32((_clamp_f32(p, 0.0, 100.0) / _F32(100)) * _F32(c))
+    x1, y1, x2, y2 = fit_box.values
+    x1, y1, x2, y2 = px(x1, w), px(y1, h), px(x2, w), px(y2, h)
+    return (x1, y1, x2, y2) if x1 < x2 and y1 < y2 else None
+
+
+def _wm_gravity1d(p, inner: int, outer: int) -> int:
+    """WatermarkDef::gravity1d (watermark.rs:59-66): f32, NOT clamped (unlike Ir4Layout's)"""
+    if (outer < inner and inner < 1) or outer < 1:
+        raise FlowError(ErrorKind.InvalidNodeParams, "Watermark fit_box does not work")
+    return _round_f32(_F32(outer - inner) * (_clamp_f32(p, 0.0, 100.0) / _F32(100)))
+
+
+def watermark_layout(frame_w: int, frame_h: int, wm_w: int, wm_h: int, watermark: Watermark) -> Optional[WatermarkDraw]:
+    """WatermarkDef::expand (flow/nodes/watermark.rs:96-205) for a frame_w x frame_h frame and a wm_w x wm_h watermark: None when the
+    node deletes itself (the frame is not strictly larger than min_canvas_*, or the fit box is under 1x1), else the draw.  Raises
+    FlowError(InvalidNodeParams) where WatermarkDef::gravity1d fails."""
+    if not (_i32(watermark.min_canvas_width or 0) < frame_w and _i32(watermark.min_canvas_height or 0) < frame_h):
+        return None
+    box = _fit_box(frame_w, frame_h, watermark.fit_box)
+    if box is None:
+        return None
+    bx1, by1, bx2, by2 = box
+    mode = watermark.fit_mode if watermark.fit_mode is not None else WatermarkConstraintMode.Within
+    crop, (w, h) = process_constraint(wm_w, wm_h, mode, (bx2 - bx1) % 2 ** 32, (by2 - by1) % 2 ** 32, watermark.gravity)
+    gx, gy = _gravity_xy(watermark.gravity)
+    x = _wm_gravity1d(gx, w, bx2 - bx1) + bx1
+    y = _wm_gravity1d(gy, h, by2 - by1) + by1
+    op = 1.0 if watermark.opacity is None else _clamp_f32(watermark.opacity, 0.0, 1.0)
+    in_w, in_h = (crop[2] - crop[0], crop[3] - crop[1]) if crop is not None else (wm_w, wm_h)
+    filt = Filter.Ginseng if (w > in_w or h > in_h) else Filter.Robidoux          # scale_render.rs:251-259, hints None
+    return WatermarkDraw(tuple(crop) if crop is not None else None, x, y, w, h, filt, float(op) if op < 1 else None)
+
+
+def riapi_watermark_placement(watermarks) -> tuple:
+    """RIAPI's layout (imageflow_riapi ir4/layout.rs:593-636): the watermarks drawn before the padding (fit box None, ImageMargins,
+    ImagePercentage) and after it (CanvasMargins, CanvasPercentage), each in the given order."""
+    wms = list(watermarks or [])
+    before = [w for w in wms if w.fit_box is None or w.fit_box.kind in (WatermarkConstraintBox.IMAGE_MARGINS, WatermarkConstraintBox.IMAGE_PERCENTAGE)]
+    after = [w for w in wms if w.fit_box is not None and w.fit_box.kind in (WatermarkConstraintBox.CANVAS_MARGINS, WatermarkConstraintBox.CANVAS_PERCENTAGE)]
+    return before, after
+
+
+_WATERMARK_DESC_DTYPE = np.dtype({
+    "names": ["draw_" + n for n, _ in ResampleDesc._fields_] + ["opacity"],
+    "formats": [np.uint64 if t is C.c_void_p else (np.uint8, (4,)) if hasattr(t, "_length_") else np.dtype(t) for _, t in ResampleDesc._fields_]
+               + [np.float32],
+    "offsets": [WatermarkDesc.draw.offset + getattr(ResampleDesc, n).offset for n, _ in ResampleDesc._fields_] + [WatermarkDesc.opacity.offset],
+    "itemsize": C.sizeof(WatermarkDesc)})
+
+
 def flow_scale_spatial(samples: np.ndarray, n: int, srgb: bool = False) -> np.ndarray:
     """flow_scale_spatial[_srgb]_{n}x{n} (c_components/lib/codecs_jpeg_idct_fast.c) applied to every 8x8 block of a plane of
     samples (H x W uint8, both multiples of 8; host memory): returns the (H/8*n) x (W/8*n) plane."""
@@ -855,6 +1153,109 @@ class Batch:
                 w.compose = BitmapCompositing.BlendWithSelf
         self._keep.append([w._keep for w in wins])
         return wins
+
+    def watermark(self, jobs, stream=None) -> list:
+        """Watermark nodes on DEVICE frames (flow/nodes/watermark.rs), byte for byte as the reference's expansion, asynchronous on
+        `stream`.  jobs: iterable of (frame, watermark window, Watermark); the watermark window is the decoded watermark (its
+        alpha_meaningful is its format) and is never written.  Each job runs watermark_layout; a job whose node deletes itself changes
+        nothing.  Jobs of one frame run in order as successive library calls (one per watermark a frame has), each call one resample per
+        distinct watermark image and one composite launch for all its frames.  Returns the frames, drawn ones BlendWithSelf from then on
+        (scale_render.rs:314).  Every layout is checked before the first call: a job the layout rejects changes nothing."""
+        jobs = list(jobs)
+        self.watermark_enqueue(self.make_watermark_descs(jobs), stream)
+        return [j[0] for j in jobs]
+
+    def make_watermark_descs(self, jobs) -> list:
+        """The library calls of watermark(jobs), prepared: [(ifb200_watermark_desc array, frames, kept objects)], one per watermark a
+        frame has.  watermark_enqueue() submits them (the frames' compose and matte are read then).  Every distinct (watermark, frame
+        size, Watermark) is laid out once, and the descriptor columns are filled from per-layout arrays, so the cost per frame is a few
+        dictionary lookups."""
+        ents, index, eidx, frames = [], {}, [], []             # one entry per distinct (watermark, frame size, spec): (src, layout) or None
+        lw = ls = None; lfw = lfh = le = -1
+        for frame, wm, spec in jobs:
+            if frame.pixel_layout != "BGRA":
+                raise FlowError(ErrorKind.InvalidArgument, "Only BGRA supported for watermarks")
+            if not (wm is lw and spec is ls and frame.w == lfw and frame.h == lfh):      # a run of one watermark costs no lookup
+                k = (id(wm), frame.w, frame.h, id(spec))
+                le = index.get(k)
+                if le is None:
+                    le = index[k] = len(ents)
+                    ents.append(self._watermark_entry(frame, wm, spec))
+                lw, ls, lfw, lfh = wm, spec, frame.w, frame.h
+            eidx.append(le)
+            frames.append(frame)
+        live = [i for i, e in enumerate(eidx) if ents[e] is not None] if any(e is None for e in ents) else range(len(jobs))
+        ptrs = [frames[i].ptr for i in live]
+        if len(set(ptrs)) == len(ptrs):                        # every frame once: one call
+            calls = [list(live)]
+        else:                                                  # the k-th watermark of a frame goes into call k
+            calls, seen = [], {}
+            for i, p in zip(live, ptrs):
+                c = seen.get(p, 0)
+                seen[p] = c + 1
+                if c == len(calls):
+                    calls.append([])
+                calls[c].append(i)
+        m = max(len(ents), 1)
+        col = {k: np.zeros(m, t) for k, t in (("in_", np.uint64), ("in_w", np.uint32), ("in_h", np.uint32), ("in_stride", np.uint32),
+                                             ("am", np.int32), ("cv_w", np.uint32), ("cv_h", np.uint32), ("x", np.uint32),
+                                             ("y", np.uint32), ("w", np.uint32), ("h", np.uint32), ("filter", np.int32), ("opacity", np.float32))}
+        for e, ent in enumerate(ents):
+            if ent is None:
+                continue
+            (src, lay), fw, fh = ent
+            for k, v in (("in_", src.ptr), ("in_w", src.w), ("in_h", src.h), ("in_stride", src.stride), ("am", bool(src.alpha_meaningful)),
+                         ("cv_w", fw), ("cv_h", fh), ("x", lay.x), ("y", lay.y), ("w", lay.w), ("h", lay.h), ("filter", int(lay.filter)),
+                         ("opacity", 1.0 if lay.opacity is None else lay.opacity)):
+                col[k][e] = v
+        e_all = np.asarray(eidx, np.int64)
+        out = []
+        for sel in calls:
+            E = e_all[np.asarray(sel, np.int64)]
+            fr = [frames[i] for i in sel]
+            a = np.zeros(len(sel), _WATERMARK_DESC_DTYPE)      # filled a column at a time: no per-field ctypes marshalling
+            for k in ("in_", "in_w", "in_h", "in_stride", "cv_w", "cv_h", "x", "y", "w", "h", "filter"):
+                a["draw_" + k] = col[k][E]
+            a["draw_alpha_meaningful"] = col["am"][E]; a["opacity"] = col["opacity"][E]
+            a["draw_canvas"] = [f.ptr for f in fr]; a["draw_cv_stride"] = [f.stride for f in fr]; a["draw_linear"] = 1
+            out.append((a, fr, [ents[e][0][0]._keep for e in set(E.tolist())]))
+        return out
+
+    @staticmethod
+    def _watermark_entry(frame: BitmapWindow, wm: BitmapWindow, spec: "Watermark"):
+        """((cropped watermark window, WatermarkDraw), frame w, frame h), or None when the node deletes itself"""
+        if wm.pixel_layout != "BGRA":
+            raise FlowError(ErrorKind.InvalidArgument, "Only BGRA supported for watermarks")
+        lay = watermark_layout(frame.w, frame.h, wm.w, wm.h, spec)
+        if lay is None:
+            return None
+        if lay.x < 0 or lay.y < 0 or lay.x + lay.w > frame.w or lay.y + lay.h > frame.h:      # scale_render.rs:236-238
+            raise FlowError(ErrorKind.InvalidNodeParams, f"DrawImageExact target rect x1={lay.x},y1={lay.y},w={lay.w},h={lay.h} "
+                                                         f"does not fit canvas size {frame.w}x{frame.h}.")
+        src = wm.window(*lay.crop) if lay.crop is not None else wm
+        if src is None:
+            raise FlowError(ErrorKind.InvalidArgument, f"crop {lay.crop} is outside the {wm.w}x{wm.h} watermark")
+        return (src, lay), frame.w, frame.h
+
+    def watermark_enqueue(self, calls, stream=None) -> None:
+        """Submits make_watermark_descs(): each call takes the frames' compose and matte as they are when it is made (a frame is
+        BlendWithSelf after its first watermark)."""
+        self_mode = BitmapCompositing.BlendWithSelf
+        for a, fr, keep in calls:
+            comp = [f.compose for f in fr]
+            if all(c is self_mode for c in comp):
+                a["draw_compose"] = 1
+            else:
+                a["draw_compose"] = [int(c) for c in comp]
+                for i, c in enumerate(comp):
+                    if c == BitmapCompositing.BlendWithMatte:
+                        a["draw_matte_bgra"][i] = tuple(fr[i].matte_bgra)
+            arr = (WatermarkDesc * len(fr)).from_buffer(a)
+            buf = C.create_string_buffer(512)
+            _check(lib().ifb200_batch_watermark(self._h, arr, len(fr), self._stream(stream), buf, 512), buf)
+            for f in fr:
+                f.compose = self_mode
+            self._keep.append(([f._keep for f in fr], keep))
 
     def flip_vertical(self, bitmap: BitmapWindow, stream=None) -> None:
         """graphics/flip.rs:10-22 on a DEVICE bitmap, in place."""

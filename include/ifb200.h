@@ -243,6 +243,20 @@ typedef struct ifb200_color_desc {
     uint32_t n_steps;
 } ifb200_color_desc;
 
+/* One watermark composite: the work of the nodes WatermarkDef::expand (flow/nodes/watermark.rs:96-205) leaves behind for one frame, after
+ * the caller has done the layout (crop, x, y, w, h, filter):
+ *   draw     the DrawImageExact of the watermark onto the frame.  draw.in is the watermark window AFTER the layout's crop (a sub-window
+ *            at any 4-byte offset), draw.canvas the frame, draw.alpha_meaningful the watermark's format, draw.compose the frame's
+ *            compositing mode going in: the library applies the Compose rule itself (ReplaceSelf is drawn as BlendWithSelf,
+ *            scale_render.rs:282-284; BlendWithSelf and BlendWithMatte stay).  color_matrix must be NULL.
+ *   opacity  Watermark.opacity.unwrap_or(1) as given: clamped to [0, 1] and, when < 1, applied as ColorFilterSrgb::Alpha (EnableTransparency
+ *            + the alpha matrix) to a private copy of the window before the draw (watermark.rs:166-172); NaN and >= 1 mean no opacity step.
+ * The caller's watermark is never written.  Afterwards the frame is BlendWithSelf (scale_render.rs:314): the caller sets that. */
+typedef struct ifb200_watermark_desc {
+    ifb200_resample_desc draw;
+    float opacity;
+} ifb200_watermark_desc;
+
 /* ---- device-resident batch API (the metric path; not in the reference) -----------------------
  * descs[i].in / .canvas are DEVICE pointers on the batch's device; color_matrix stays a HOST pointer.
  * enqueue is asynchronous on `cuda_stream`, a cudaStream_t with the usual CUDA meaning (NULL = the legacy
@@ -301,6 +315,18 @@ int  ifb200_batch_orient(ifb200_batch* b, const ifb200_orient_desc* d, size_t n,
  * IFB200_ERR_NOT_IMPLEMENTED.  There is no host-buffer variant: on a host bitmap one pass of the reference's own loop costs less than
  * the trip to the GPU and back. */
 int  ifb200_batch_color_chain(ifb200_batch* b, const ifb200_color_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
+/* Watermarks (ifb200_watermark_desc) on n DEVICE frames, byte for byte as the node-by-node expansion (copy, Alpha, DrawImageExact).  Jobs
+ * whose watermark resamples to the same premultiplied working-space image F (same source window, format, applied opacity, size, filter,
+ * sharpen and working space) share ONE resample: the existing generic H pass and a V pass that stores F, one pair per distinct geometry;
+ * then ONE composite launch writes every job's rectangle from its F.  Kernel launches per call: 1 + 2 x (distinct geometries), plus 1 when
+ * some job has an opacity (the colour chain on the private copies); none when no job has pixels.  Device memory: the F of a call's
+ * distinct watermarks (16 bytes per pixel of each) and their private copies are held at most 1 GiB at a time (plus the H pass's
+ * intermediate, also at most 1 GiB, and a single F larger than that alone): a call that needs more is run as consecutive chunks of its
+ * groups, each with the launches above.  Asynchronous on `cuda_stream`.  No two
+ * jobs of a call may write the same pixel (not checked): several watermarks on one frame are successive calls.  A job with w or h = 0 is
+ * skipped unchecked; every other descriptor is checked (as ifb200_batch_enqueue checks it, plus 4-byte aligned pointers and a NULL
+ * colour matrix) and plans are built before anything is enqueued, so an error means nothing is written.  There is no host-buffer variant. */
+int  ifb200_batch_watermark(ifb200_batch* b, const ifb200_watermark_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
 int  ifb200_batch_sync(ifb200_batch* b, char* err, size_t err_cap);
 void ifb200_batch_destroy(ifb200_batch* b);
 /* knobs / introspection (benchmarks, tests) */

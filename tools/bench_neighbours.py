@@ -2,7 +2,8 @@
 """Measurement of the SURVEY.md section 8(f) neighbours of the resample path that are built: transpose, flips, white balance, detect_content
 and rounded corners; `bench_neighbours.py canvas` measures the canvas operations alone (canvas_rows), `bench_neighbours.py orient`
 the one-gather orientation against the reference's expansion into transposes and flips (orient_rows), `bench_neighbours.py color` the
-colour chains against the reference's node-by-node expansion (color_rows)
+colour chains against the reference's node-by-node expansion (color_rows), `bench_neighbours.py watermark` the watermark composites
+against the node-by-node expansion and the best existing route (watermark_rows)
 (the reference benchmarks transposes at 4K / 8K in benches/bench_graphics.rs:9-62).  Inputs resident in HBM, CUDA events on
 the launching stream, >= 3 warm-up calls; a set of 64 different images per size (>= 2 GB, far larger than L2) is cycled so that
 no call finds its data in cache.  One JSON line per (operation, size) with the HBM roofline of the kernel: algorithmic
@@ -455,8 +456,147 @@ def color_rows():
     b.sync()
 
 
+def _device_ms(fn, reps=10):
+    """GPU time per call of fn: the durations of every kernel and copy it enqueues, summed over a torch.profiler trace of reps calls"""
+    from torch.profiler import ProfilerActivity, profile
+    fn(); torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(reps):
+            fn()
+        torch.cuda.synchronize()
+    us = sum(getattr(e, "self_device_time_total", None) or getattr(e, "self_cuda_time_total", 0) for e in prof.key_averages())
+    return us / 1e3 / reps
+
+
+def watermark_rows():
+    """Watermarks (Batch.watermark) on frames resident in HBM, each route timed in five trials (median, smallest, largest).
+    (a) 1024 512x512 thumbnails, a 400x100 cut-out logo, Within into ImagePercentage(0, 0, 90, 90), gravity (100, 100), opacity 0.9
+        (visuals/watermark.rs test_watermark_image_small): one call; the node-by-node expansion (per frame a copy of the logo, the Alpha
+        chain on it, one resample); and the best existing route (the Alpha chain once on one copy, then ONE batch_enqueue of 1024 jobs
+        whose descriptors are built beforehand).  The host wall time inside the one call is reported apart.
+    (b) 64 3840x2160 frames, each with a 1920x1080 watermark fitted to the whole canvas (CanvasPercentage(0, 0, 100, 100), Fit): one
+        call and one batch_enqueue of the 64 draws, against a torch copy of the algorithmic bytes, 8 per composited pixel (4 read, 4
+        written).  F (16 bytes per pixel, written once and read once per frame) is reported apart.
+    Each row checks a frame of the one call against the other route, bit for bit."""
+    card = _card()
+    pk, src = peak()
+    b = ifb.Batch(0)
+    stream = torch.cuda.current_stream().cuda_stream
+    M, B, G = ifb.WatermarkConstraintMode, ifb.WatermarkConstraintBox, ifb.ConstraintGravity
+    from imageflow_b200 import synth
+
+    def trials(fn, reps):
+        t = sorted(_time_ms(fn, reps=reps) for _ in range(5))
+        return t[2], [t[0], t[-1]]
+
+    # (a)
+    n, fw = 1024, 512
+    frames = torch.randint(0, 256, (n, fw, fw, 4), dtype=torch.uint8, device="cuda")
+    base = frames.clone()
+    logo = synth.cutout_torch(400, 100, 3)
+    spec = ifb.Watermark(fit_box=B.image_percentage(0, 0, 90, 90), fit_mode=M.Within, gravity=G.percentage(100, 100), opacity=0.9)
+    wins = [ifb.BitmapWindow.from_torch(frames[i]) for i in range(n)]
+    lw = ifb.BitmapWindow.from_torch(logo, alpha_meaningful=True)
+    draw = ifb.watermark_layout(fw, fw, 400, 100, spec)
+    params = ifb.ScaleAndRenderParams(x=draw.x, y=draw.y, w=draw.w, h=draw.h, interpolation_filter=draw.filter)
+
+    def one_call():
+        for w in wins:
+            w.compose = ifb.BitmapCompositing.BlendWithSelf
+        b.watermark([(w, lw, spec) for w in wins], stream)
+
+    def expansion():
+        for w in wins:
+            c = logo.clone()
+            cw = ifb.BitmapWindow.from_torch(c, alpha_meaningful=True)
+            b.color_chain([(cw, ifb.ColorFilterSrgb.alpha(draw.opacity))], stream)
+            w.compose = ifb.BitmapCompositing.BlendWithSelf
+            b.scale_and_render_many([(cw, w, params)], stream)
+
+    copy = logo.clone()
+    cwin = ifb.BitmapWindow.from_torch(copy, alpha_meaningful=True)
+    for w in wins:
+        w.compose = ifb.BitmapCompositing.BlendWithSelf
+    descs, keep = b.make_descs([(cwin, w, params) for w in wins])
+
+    def best_existing():
+        copy.copy_(logo)
+        b.color_chain([(cwin, ifb.ColorFilterSrgb.alpha(draw.opacity))], stream)
+        b.enqueue(descs, stream)
+
+    prepared = b.make_watermark_descs([(w, lw, spec) for w in wins])
+
+    def library_call():                                      # the library alone: descriptors built beforehand, as best_existing's
+        for w in wins:
+            w.compose = ifb.BitmapCompositing.BlendWithSelf
+        b.watermark_enqueue(prepared, stream)
+
+    before = b.kernel_launches
+    one_call()
+    launches = b.kernel_launches - before
+    ms_one, mm_one = trials(one_call, 10)
+    ms_lib, mm_lib = trials(library_call, 10)
+    host_lib = sorted(_time_event_and_host_ms(library_call)[1] for _ in range(5))[2]
+    host = sorted(_time_event_and_host_ms(one_call)[1] for _ in range(5))[2]
+    ms_exp, mm_exp = trials(expansion, 1)
+    ms_best, mm_best = trials(best_existing, 10)
+    # device time alone (kernels and copies, summed from a torch.profiler trace taken after the timed trials): row (a) is bound by host
+    # time on every route, so the event times above do not show what the GPU spends
+    dev_one, dev_best = _device_ms(one_call), _device_ms(best_existing)
+    frames.copy_(base); one_call(); got = frames.clone()
+    frames.copy_(base); best_existing(); ok = bool(torch.equal(got, frames))
+    alg = n * draw.w * draw.h * 8
+    print(json.dumps({"op": "watermark", "row": f"a_{n}x{fw}x{fw}_logo_400x100_within_90pct_opacity_0.9", "one_call_ms": ms_one,
+                      "one_call_ms_min_max": mm_one, "host_wall_ms_inside_one_call": host,
+                      "prebuilt_descriptors_call_ms": ms_lib, "prebuilt_descriptors_call_ms_min_max": mm_lib,
+                      "host_wall_ms_inside_prebuilt_call": host_lib, "prebuilt_call_vs_best_existing": ms_best / ms_lib, "expansion_ms": ms_exp,
+                      "expansion_ms_min_max": mm_exp, "best_existing_ms": ms_best, "best_existing_ms_min_max": mm_best,
+                      "one_call_vs_best_existing": ms_best / ms_one,
+                      "device_ms_one_call": dev_one, "device_ms_best_existing": dev_best, "one_call_vs_expansion": ms_exp / ms_one, "launches_per_call": launches,
+                      "draw": [draw.x, draw.y, draw.w, draw.h], "algorithmic_bytes": alg, "bit_exact_vs_best_existing": ok, **card}), flush=True)
+    del frames, base, wins, descs, keep
+    torch.cuda.empty_cache()
+
+    # (b)
+    n, w, h = 64, 3840, 2160
+    frames = (torch.randn((n, h, w, 4), device="cuda") * 40 + 128).clamp_(0, 255).to(torch.uint8)
+    wm = synth.cutout_torch(1920, 1080, 5)
+    spec = ifb.Watermark(fit_box=B.canvas_percentage(0, 0, 100, 100), fit_mode=M.Fit)
+    wins = [ifb.BitmapWindow.from_torch(frames[i]) for i in range(n)]
+    ww = ifb.BitmapWindow.from_torch(wm, alpha_meaningful=True)
+    draw = ifb.watermark_layout(w, h, 1920, 1080, spec)
+    params = ifb.ScaleAndRenderParams(x=draw.x, y=draw.y, w=draw.w, h=draw.h, interpolation_filter=draw.filter)
+    for x in wins:
+        x.compose = ifb.BitmapCompositing.BlendWithSelf
+    descs, keep = b.make_descs([(ww, x, params) for x in wins])
+
+    def one_call_b():
+        for x in wins:
+            x.compose = ifb.BitmapCompositing.BlendWithSelf
+        b.watermark([(x, ww, spec) for x in wins], stream)
+
+    ms_one, mm_one = trials(one_call_b, 3)
+    ms_enq, mm_enq = trials(lambda: b.enqueue(descs, stream), 3)
+    keep0 = frames[0].clone()
+    one_call_b(); got = frames[0].clone(); frames[0].copy_(keep0)
+    d0, k0 = b.make_descs([(ww, wins[0], params)])
+    b.enqueue(d0, stream); ok = bool(torch.equal(got, frames[0]))
+    alg = n * draw.w * draw.h * 8
+    cm = _copy_ceiling_ms(alg)
+    print(json.dumps({"op": "watermark", "row": f"b_{n}x{w}x{h}_watermark_1920x1080_fit_canvas", "one_call_ms": ms_one,
+                      "one_call_ms_min_max": mm_one, "batch_enqueue_ms": ms_enq, "batch_enqueue_ms_min_max": mm_enq,
+                      "one_call_vs_batch_enqueue": ms_enq / ms_one, "algorithmic_bytes": alg, "achieved_gbs": alg / ms_one / 1e6,
+                      "frac_of_peak": alg / ms_one / 1e6 / pk, "peak_gbs": pk, "peak_source": src, "torch_copy_same_bytes_ms": cm,
+                      "frac_of_torch_copy": cm / ms_one, "f_bytes_written_once": draw.w * draw.h * 16,
+                      "f_bytes_read_per_call": n * draw.w * draw.h * 16, "draw": [draw.x, draw.y, draw.w, draw.h],
+                      "bit_exact_vs_batch_enqueue": ok, **card}), flush=True)
+    b.sync()
+
+
 if __name__ == "__main__":
-    if sys.argv[1:] == ["canvas"]:
+    if sys.argv[1:] == ["watermark"]:
+        watermark_rows()
+    elif sys.argv[1:] == ["canvas"]:
         canvas_rows()
     elif sys.argv[1:] == ["orient"]:
         orient_rows()
