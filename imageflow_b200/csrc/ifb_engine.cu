@@ -14,6 +14,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -772,14 +773,15 @@ const HvTmap& tmap_for(ifb200_batch* b, const ifb200_resample_desc& d, uint32_t*
     return b->tmaps.emplace(key, h).first->second;
 }
 
-// frees a stream-ordered allocation when the scope is left by an exception (the normal path frees it itself)
+// frees a stream-ordered allocation on its stream when the scope is left, after the work that uses it has been enqueued or when an
+// exception leaves the scope
 struct AsyncFree {
     void* p = nullptr; cudaStream_t st = nullptr;
     ~AsyncFree() { if (p) cudaFreeAsync(p, st); }
-    void release() { p = nullptr; }
 };
 
 void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n, cudaStream_t st) {
+    if (!descs && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
     if (n == 0) return;
     Tick tk_all(b->prof.enqueue);
     host_tables();
@@ -994,34 +996,60 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
     st = user_stream;
 }
 
+// The argument checks of a BGRA window, shared by the device and the host-buffer form of each operation: a null pointer, or a stride
+// below a row or not a multiple of 4, is an argument error.  Returns false for an empty window (nothing to do).
+bool bgra_window(const void* px, uint32_t w, uint32_t h, uint32_t stride) {
+    if (!px) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null bitmap pointer");
+    if (w == 0 || h == 0) return false;
+    if (stride < w * 4ull || (stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "stride smaller than a BGRA row or not a multiple of 4");
+    return true;
+}
+
+// The work lists of one launch: host arrays at 256-byte aligned offsets in ONE stream-ordered device allocation on `st`, filled by ONE
+// copy through a pinned staging slot, and `tail` bytes after them that are allocated but not copied.  off[k] is the offset of array k,
+// off[number of arrays] that of the tail.  The allocation is freed on `st` when the object goes out of scope, after the launches that
+// read it have been enqueued.
+struct WorkUpload {
+    struct Part { const void* p; size_t bytes; };
+    AsyncFree mem;
+    std::vector<size_t> off;
+    WorkUpload(ifb200_batch* b, cudaStream_t st, std::initializer_list<Part> parts, size_t tail = 0) : mem{nullptr, st} {
+        size_t end = 0;
+        for (const Part& q : parts) { off.push_back((end + 255) / 256 * 256); end = off.back() + q.bytes; }
+        off.push_back((end + 255) / 256 * 256);
+        cudaEvent_t ev;
+        uint8_t* h = static_cast<uint8_t*>(b->stage(end, &ev));
+        const Part* q = parts.begin();
+        for (size_t k = 0; k < parts.size(); ++k) if (q[k].bytes) memcpy(h + off[k], q[k].p, q[k].bytes);
+        CUDA_OK(cudaMallocAsync(&mem.p, off.back() + tail, st));
+        CUDA_OK(cudaMemcpyAsync(mem.p, h, end, cudaMemcpyHostToDevice, st));
+        CUDA_OK(cudaEventRecord(ev, st));
+    }
+    template <class T> T* at(size_t k) const { return reinterpret_cast<T*>(static_cast<uint8_t*>(mem.p) + off[k]); }
+};
+template <class T> WorkUpload::Part part(const std::vector<T>& v) { return {v.data(), v.size() * sizeof(T)}; }
+
 void color_matrix_locked(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, const float* m, cudaStream_t st) {
-    if (!dev_px || !m) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
-    if (w == 0 || h == 0) return;
-    if (stride < w * 4ull || (stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "bad stride");
+    if (!m) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null matrix pointer");
+    if (!bgra_window(dev_px, w, h, stride)) return;
+    const uint64_t total = (uint64_t)w * h;
+    if (total > 0xffffffffull) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "bitmap too large");
     DeviceScope dev_scope_(b->device);
-    cudaEvent_t ev;
-    float* hm = static_cast<float*>(b->stage(20 * sizeof(float), &ev));
+    float hm[20];
     for (int c = 0; c < 4; ++c) {
         for (int k = 0; k < 4; ++k) hm[c * 5 + k] = m[k * 5 + c];
         hm[c * 5 + 4] = m[4 * 5 + c] * 255.0f;                 // color_matrix.rs:9-12
     }
-    float* dm = nullptr;
-    CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&dm), 20 * sizeof(float), st));
-    CUDA_OK(cudaMemcpyAsync(dm, hm, 20 * sizeof(float), cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaEventRecord(ev, st));
-    const uint64_t total = (uint64_t)w * h;
-    if (total > 0xffffffffull) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "bitmap too large");
+    WorkUpload up(b, st, {{hm, sizeof hm}});
     const unsigned blocks = (unsigned)std::min<uint64_t>((total + 255) / 256, (uint64_t)b->sm_count * 16);
-    color_matrix_kernel<<<blocks, 256, 0, st>>>(dev_px, w, h, stride, dm);
+    color_matrix_kernel<<<blocks, 256, 0, st>>>(dev_px, w, h, stride, up.at<const float>(0));
     CUDA_OK(cudaGetLastError());
     b->launches++;
-    CUDA_OK(cudaFreeAsync(dm, st));
 }
 
 void apply_matte_locked(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, const uint8_t* matte, cudaStream_t st) {
-    if (!dev_px || !matte) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
-    if (w == 0 || h == 0) return;
-    if (stride < w * 4ull || (stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "bad stride");
+    if (!matte) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null matte pointer");
+    if (!bgra_window(dev_px, w, h, stride)) return;
     const uint64_t total = (uint64_t)w * h;
     if (total > 0xffffffffull) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "bitmap too large");
     DeviceScope dev_scope_(b->device);
@@ -1039,11 +1067,8 @@ constexpr int kHostSlots = 3;
 // transpose.rs:95-121 + the bounds checks of transpose.rs:46-79 (strides in bytes here)
 void transpose_locked(ifb200_batch* b, const uint8_t* from, uint32_t from_stride, uint32_t w, uint32_t h, uint8_t* to, uint32_t to_stride,
                       cudaStream_t st) {
-    if (!from || !to) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null bitmap pointer");
-    if (w == 0 || h == 0) return;
-    if ((from_stride & 3) || (to_stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "strides must be multiples of 4 bytes");
-    if (from_stride < w * 4ull) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "from_stride(%u) < width(%u)", from_stride / 4, w);
-    if (to_stride < h * 4ull) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "to_stride(%u) < height(%u)", to_stride / 4, h);
+    if (!to) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null bitmap pointer");
+    if (!bgra_window(from, w, h, from_stride) || !bgra_window(to, h, w, to_stride)) return;      // `to` is h x w: empty when `from` is
     DeviceScope dev_scope_(b->device);
     const uint32_t rows_per_launch = 65535u * 32u;           // grid.y is bounded; bitmaps are not
     for (uint32_t y0 = 0; y0 < h; y0 += rows_per_launch) {
@@ -1055,9 +1080,7 @@ void transpose_locked(ifb200_batch* b, const uint8_t* from, uint32_t from_stride
     }
 }
 void flip_locked(ifb200_batch* b, bool vertical, uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, cudaStream_t st) {
-    if (!px) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null bitmap pointer");
-    if (w == 0 || h == 0) return;
-    if (stride < w * 4ull || (stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "stride smaller than a BGRA row or not a multiple of 4");
+    if (!bgra_window(px, w, h, stride)) return;
     const bool v4 = (w % 4 == 0) && (stride % 16 == 0) && ((uintptr_t)px % 16 == 0);       // four pixels per access
     const uint32_t we = v4 ? w / 4 : w;
     const uint64_t elems = vertical ? (uint64_t)(h / 2) * we : (uint64_t)(v4 ? (we + 1) / 2 : we / 2) * h;
@@ -1096,9 +1119,7 @@ void block_scale_locked(ifb200_batch* b, const uint8_t* in, uint32_t in_stride, 
 // flow/nodes/white_balance.rs:93-121 (WhiteBalanceSrgbMutDef::mutate): histograms, area thresholds, byte maps, remap.
 // threshold < 0 stands for None (-> 0.006f32, white_balance.rs:76-77); both thresholds are the same value (:114).
 void white_balance_locked(ifb200_batch* b, uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, float threshold, cudaStream_t st) {
-    if (!px) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null bitmap pointer");
-    if (w == 0 || h == 0) return;
-    if (stride < w * 4ull || (stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "stride smaller than a BGRA row or not a multiple of 4");
+    if (!bgra_window(px, w, h, stride)) return;
     if (threshold != threshold) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "threshold is NaN");
     DeviceScope dev_scope_(b->device);
     const double low = (double)(threshold < 0.0f ? 0.006f : threshold);      // f64::from(f32)
@@ -1122,13 +1143,19 @@ void white_balance_locked(ifb200_batch* b, uint8_t* px, uint32_t w, uint32_t h, 
     b->launches += 3;
 }
 
+// The limits of the code map's bitmap and threshold (an empty bitmap is an error here)
+void whitespace_check(const uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, uint32_t threshold) {
+    if (!bgra_window(px, w, h, stride)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "empty bitmap");
+    if (w > 0x7fffffffu || h > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "oversized bitmap");
+    if (threshold > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "threshold out of range");
+}
+
 // The per-pixel code map of detect_content (layout: ifb_whitespace.h) of a DEVICE bitmap into a DEVICE buffer of w*h bytes; asynchronous.
 void whitespace_codes_locked(ifb200_batch* b, const uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, int alpha_meaningful,
                              uint32_t threshold, uint8_t* dcodes, cudaStream_t st) {
-    if (!px || !dcodes) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
-    if (w == 0 || h == 0 || w > 0x7fffffffu || h > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "empty or oversized bitmap");
-    if (stride < w * 4ull || (stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "stride smaller than a BGRA row or not a multiple of 4");
-    if (threshold > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "threshold out of range");
+    if (!dcodes) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
+    whitespace_check(px, w, h, stride, threshold);
+    DeviceScope dev_scope_(b->device);
     // grid.y is bounded: tall bitmaps go in chunks of rows (a chunk's first and last rows look one row up / down: the kernel
     // takes the whole bitmap and the chunk's first row)
     const uint32_t rows_per_launch = 65535u * 8u;
@@ -1145,10 +1172,8 @@ void whitespace_codes_locked(ifb200_batch* b, const uint8_t* px, uint32_t w, uin
 // back to the host, the reference's window walk over it there.  Returns a rectangle, so it synchronises `st`.
 void detect_content_locked(ifb200_batch* b, const uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, int alpha_meaningful,
                            uint32_t threshold, cudaStream_t st, uint32_t rect[4]) {
-    if (!px || !rect) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
-    if (w == 0 || h == 0 || w > 0x7fffffffu || h > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "empty or oversized bitmap");
-    if (stride < w * 4ull || (stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "stride smaller than a BGRA row or not a multiple of 4");
-    if (threshold > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "threshold out of range");
+    if (!rect) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
+    whitespace_check(px, w, h, stride, threshold);
     rect[0] = 0; rect[1] = 0; rect[2] = w; rect[3] = h;
     if (w < 3 || h < 3) return;                              // whitespace.rs:288-290
     DeviceScope dev_scope_(b->device);
@@ -1165,79 +1190,27 @@ void detect_content_locked(ifb200_batch* b, const uint8_t* px, uint32_t w, uint3
     if (!ifb::detect_content_from_codes(codes, w, h, rect, nullptr)) IFB_THROW(IFB200_ERR_INVALID_STATE, "whitespace walk failed");
 }
 
-// flow_bitmap_bgra_clear_around_rounded_corners (graphics/rounded_corners.rs:187-346).  Argument checks of one job; degenerate radii
-// are not errors (the planner gives them the reference's meaning).
-void round_corners_validate(const ifb200_round_corners_desc& d) {
-    if (d.mode < IFB200_CORNERS_PERCENTAGE || d.mode > IFB200_CORNERS_PIXELS_CUSTOM) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "unknown corners mode %d", d.mode);
-    if (d.w == 0 || d.h == 0) return;
-    if (!d.px) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null bitmap pointer");
-    if (d.stride < d.w * 4ull || (d.stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "stride smaller than a BGRA row or not a multiple of 4");
-    if ((uint64_t)d.w * d.h > 0xffffffffull) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "bitmap too large");
-}
-// the planned job of a validated, non-empty descriptor, on bitmap (px, stride)
-ifb::RcJob round_corners_job(const ifb200_round_corners_desc& d, uint8_t* px, uint32_t stride) {
-    ifb::RcJob job{};
-    if (!ifb::round_corners_plan(d.mode, d.radius, d.w, d.h, &job)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "unknown corners mode %d", d.mode);
-    job.px = px; job.stride = stride;
-    job.matte = (uint32_t)d.matte_bgra[0] | ((uint32_t)d.matte_bgra[1] << 8) | ((uint32_t)d.matte_bgra[2] << 16) | ((uint32_t)d.matte_bgra[3] << 24);
-    return job;
-}
-// Jobs and their cover rectangles cut into CTA tiles of at most kRcTilePixels pixels
-struct RcWork {
-    std::vector<ifb::RcJob> jobs; std::vector<ifb::RcTile> tiles;
-    void add(const ifb::RcJob& job, const std::vector<ifb::RcRect>& rects) {
-        const uint32_t j = (uint32_t)jobs.size();
-        jobs.push_back(job);
-        for (const auto& r : rects) {
-            const uint64_t area = (uint64_t)r.w * r.h;
-            for (uint64_t f = 0; f < area; f += ifb::kRcTilePixels)
-                tiles.push_back({j, r.x0, r.y0, r.w, (uint32_t)f, (uint32_t)std::min<uint64_t>(ifb::kRcTilePixels, area - f)});
-        }
-    }
-};
-// The job and tile lists of one flat launch in one stream-ordered device allocation on `st` (staged through pinned memory): returns
-// it, with the jobs at offset 0 and the tiles at *tiles_at.  The caller launches, then frees it on `st`.
-template <class J, class T>
-uint8_t* upload_work(ifb200_batch* b, const std::vector<J>& jobs, const std::vector<T>& tiles, cudaStream_t st, size_t* tiles_at) {
-    if (tiles.size() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
-    const size_t jb = (jobs.size() * sizeof(J) + 255) / 256 * 256, tb = tiles.size() * sizeof(T);
-    cudaEvent_t ev;
-    uint8_t* hbuf = static_cast<uint8_t*>(b->stage(jb + tb, &ev));
-    memcpy(hbuf, jobs.data(), jobs.size() * sizeof(J));
-    memcpy(hbuf + jb, tiles.data(), tb);
-    uint8_t* dbuf = nullptr;
-    CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&dbuf), jb + tb, st));
-    AsyncFree dbuf_guard{dbuf, st};
-    CUDA_OK(cudaMemcpyAsync(dbuf, hbuf, jb + tb, cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaEventRecord(ev, st));
-    dbuf_guard.release();
-    *tiles_at = jb;
-    return dbuf;
-}
-// ONE launch for every tile of `wk`, asynchronous on `st` (none when no job touches a pixel)
-void round_corners_launch(ifb200_batch* b, const RcWork& wk, cudaStream_t st) {
+// ONE launch of round_corners_kernel for every tile of `wk`, asynchronous on `st` (none when no job touches a pixel)
+void round_corners_launch(ifb200_batch* b, const ifb::RcWork& wk, cudaStream_t st) {
     if (wk.tiles.empty()) return;
+    if (wk.tiles.size() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
     DeviceScope dev_scope_(b->device);
-    size_t jb = 0;
-    uint8_t* dbuf = upload_work(b, wk.jobs, wk.tiles, st, &jb);
-    AsyncFree dbuf_guard{dbuf, st};
-    round_corners_kernel<<<(unsigned)wk.tiles.size(), ifb::kRcThreads, 0, st>>>(reinterpret_cast<const ifb::RcJob*>(dbuf),
-                                                                              reinterpret_cast<const ifb::RcTile*>(dbuf + jb), b->tables);
+    WorkUpload up(b, st, {part(wk.jobs), part(wk.tiles)});
+    round_corners_kernel<<<(unsigned)wk.tiles.size(), ifb::kRcThreads, 0, st>>>(up.at<const ifb::RcJob>(0), up.at<const ifb::RcTile>(1), b->tables);
     CUDA_OK(cudaGetLastError());
     b->launches++;
 }
+
+// The rounded corners of ifb200_batch_round_corners (ifb_round_corners.h): every descriptor is checked before anything is planned or
+// enqueued, then all jobs run in ONE launch.
 void round_corners_locked(ifb200_batch* b, const ifb200_round_corners_desc* d, size_t n, cudaStream_t st) {
     if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
-    for (size_t i = 0; i < n; ++i) round_corners_validate(d[i]);           // all-or-nothing, before any device use
-    RcWork wk;
-    std::vector<ifb::RcRect> rects;
     for (size_t i = 0; i < n; ++i) {
-        if (d[i].w == 0 || d[i].h == 0) continue;
-        const ifb::RcJob job = round_corners_job(d[i], d[i].px, d[i].stride);
-        rects.clear();
-        ifb::round_corners_cover(job, rects);
-        wk.add(job, rects);
+        const std::string why = ifb::round_corners_check(d[i]);
+        if (!why.empty()) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "round corners job %zu: %s", i, why.c_str());
     }
+    ifb::RcWork wk;
+    for (size_t i = 0; i < n; ++i) ifb::round_corners_plan(d[i], wk);
     round_corners_launch(b, wk, st);
 }
 
@@ -1252,12 +1225,10 @@ void canvas_locked(ifb200_batch* b, const ifb200_canvas_desc* d, size_t n, cudaS
     ifb::CvWork wk;
     for (size_t i = 0; i < n; ++i) ifb::canvas_plan(d[i], wk);
     if (wk.tiles.empty()) return;
+    if (wk.tiles.size() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
     DeviceScope dev_scope_(b->device);
-    size_t tb = 0;
-    uint8_t* dbuf = upload_work(b, wk.items, wk.tiles, st, &tb);
-    AsyncFree dbuf_guard{dbuf, st};
-    canvas_kernel<<<(unsigned)wk.tiles.size(), ifb::kCvThreads, 0, st>>>(reinterpret_cast<const ifb::CvItem*>(dbuf),
-                                                                       reinterpret_cast<const ifb::CvTile*>(dbuf + tb));
+    WorkUpload up(b, st, {part(wk.items), part(wk.tiles)});
+    canvas_kernel<<<(unsigned)wk.tiles.size(), ifb::kCvThreads, 0, st>>>(up.at<const ifb::CvItem>(0), up.at<const ifb::CvTile>(1));
     CUDA_OK(cudaGetLastError());
     b->launches++;
 }
@@ -1275,11 +1246,8 @@ void orient_locked(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, cudaS
     if (wk.items.empty()) return;
     if (wk.ctas() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
     DeviceScope dev_scope_(b->device);
-    size_t fb = 0;
-    uint8_t* dbuf = upload_work(b, wk.items, wk.first, st, &fb);
-    AsyncFree dbuf_guard{dbuf, st};
-    orient_kernel<<<(unsigned)wk.ctas(), ifb::kOrThreads, 0, st>>>(reinterpret_cast<const ifb::OrItem*>(dbuf),
-                                                                 reinterpret_cast<const uint32_t*>(dbuf + fb), (uint32_t)wk.items.size());
+    WorkUpload up(b, st, {part(wk.items), part(wk.first)});
+    orient_kernel<<<(unsigned)wk.ctas(), ifb::kOrThreads, 0, st>>>(up.at<const ifb::OrItem>(0), up.at<const uint32_t>(1), (uint32_t)wk.items.size());
     CUDA_OK(cudaGetLastError());
     b->launches++;
 }
@@ -1299,32 +1267,14 @@ void color_chain_locked(ifb200_batch* b, const ifb200_color_desc* d, size_t n, c
     if (wk.jobs.empty()) return;
     if (wk.ctas() > 0x7fffffffu || wk.wb_ctas() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
     DeviceScope dev_scope_(b->device);
-    auto at = [](size_t x) { return (x + 255) / 256 * 256; };
-    const size_t o_first = at(wk.jobs.size() * sizeof(ifb::ClJob)), o_wb = o_first + at(wk.first.size() * 4),
-                 o_wbf = o_wb + at(wk.wb_jobs.size() * sizeof(ifb::ClJob)), o_segs = o_wbf + at(wk.wb_first.size() * 4),
-                 o_tab = o_segs + at(wk.segs.size() * sizeof(ifb::ClSeg)), o_mat = o_tab + at(wk.tables.size()),
-                 o_hist = o_mat + at(wk.mats.size() * sizeof(float)), hist_bytes = wk.wb_jobs.size() * 768 * sizeof(unsigned long long);
-    cudaEvent_t ev;
-    uint8_t* h = static_cast<uint8_t*>(b->stage(o_hist, &ev));
-    auto put = [&](size_t off, const void* src, size_t bytes) { if (bytes) memcpy(h + off, src, bytes); };
-    put(0, wk.jobs.data(), wk.jobs.size() * sizeof(ifb::ClJob));
-    put(o_first, wk.first.data(), wk.first.size() * 4);
-    put(o_wb, wk.wb_jobs.data(), wk.wb_jobs.size() * sizeof(ifb::ClJob));
-    put(o_wbf, wk.wb_first.data(), wk.wb_first.size() * 4);
-    put(o_segs, wk.segs.data(), wk.segs.size() * sizeof(ifb::ClSeg));
-    put(o_tab, wk.tables.data(), wk.tables.size());
-    put(o_mat, wk.mats.data(), wk.mats.size() * sizeof(float));
-    uint8_t* dbuf = nullptr;
-    CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&dbuf), o_hist + hist_bytes, st));
-    AsyncFree dbuf_guard{dbuf, st};
-    CUDA_OK(cudaMemcpyAsync(dbuf, h, o_hist, cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaEventRecord(ev, st));
-    ClDev a{reinterpret_cast<const ifb::ClJob*>(dbuf), reinterpret_cast<const uint32_t*>(dbuf + o_first), (uint32_t)wk.jobs.size(),
-            reinterpret_cast<const ifb::ClSeg*>(dbuf + o_segs), dbuf + o_tab, reinterpret_cast<const float*>(dbuf + o_mat),
-            reinterpret_cast<unsigned long long*>(dbuf + o_hist)};
+    const size_t hist_bytes = wk.wb_jobs.size() * 768 * sizeof(unsigned long long);
+    WorkUpload up(b, st, {part(wk.jobs), part(wk.first), part(wk.wb_jobs), part(wk.wb_first), part(wk.segs), part(wk.tables), part(wk.mats)},
+                  hist_bytes);
+    ClDev a{up.at<const ifb::ClJob>(0), up.at<const uint32_t>(1), (uint32_t)wk.jobs.size(), up.at<const ifb::ClSeg>(4), up.at<uint8_t>(5),
+            up.at<const float>(6), up.at<unsigned long long>(7)};
     if (!wk.wb_jobs.empty()) {
         ClDev w = a;
-        w.jobs = reinterpret_cast<const ifb::ClJob*>(dbuf + o_wb); w.first = reinterpret_cast<const uint32_t*>(dbuf + o_wbf);
+        w.jobs = up.at<const ifb::ClJob>(2); w.first = up.at<const uint32_t>(3);
         w.n = (uint32_t)wk.wb_jobs.size();
         CUDA_OK(cudaMemsetAsync(w.hist, 0, hist_bytes, st));
         color_hist_kernel<<<(unsigned)wk.wb_ctas(), ifb::kClThreads, 0, st>>>(w);
@@ -1410,18 +1360,7 @@ void watermark_locked(ifb200_batch* b, const ifb200_watermark_desc* d, size_t n,
                 }
     }
     for (uint32_t g = 0; g < ng; ++g) wk.groups[g].f = reinterpret_cast<const float*>(scratch + f_off[g]);
-    // the plan goes up in one copy
-    const size_t o_jobs = at(ng * sizeof(ifb::WmGroup)), o_h = o_jobs + at(wk.jobs.size() * sizeof(ifb::WmJob)), total = o_h + ng * sizeof(JobDev);
-    cudaEvent_t ev;
-    uint8_t* h = static_cast<uint8_t*>(b->stage(total, &ev));
-    memcpy(h, wk.groups.data(), ng * sizeof(ifb::WmGroup));
-    memcpy(h + o_jobs, wk.jobs.data(), wk.jobs.size() * sizeof(ifb::WmJob));
-    memcpy(h + o_h, hjobs.data(), ng * sizeof(JobDev));
-    uint8_t* dbuf = nullptr;
-    CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&dbuf), total, st));
-    AsyncFree dbuf_guard{dbuf, st};
-    CUDA_OK(cudaMemcpyAsync(dbuf, h, total, cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaEventRecord(ev, st));
+    WorkUpload up(b, st, {part(wk.groups), part(wk.jobs), part(hjobs)});      // the plan goes up in one copy
     std::vector<ifb200_color_step> steps(2 * ng);
     for (const Chunk& c : chunks) {
         // 1. opacity: private copies, then the existing colour chain on them (one launch)
@@ -1448,7 +1387,7 @@ void watermark_locked(ifb200_batch* b, const ifb200_watermark_desc* d, size_t n,
             float4* inter = nullptr;
             CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&inter), per * chunk, st));
             AsyncFree inter_guard{inter, st};
-            const JobDev* hj = reinterpret_cast<const JobDev*>(dbuf + o_h) + hpos[g0];
+            const JobDev* hj = up.at<const JobDev>(2) + hpos[g0];
             float4* fg = reinterpret_cast<float4*>(scratch + f_off[g0]);
             for (size_t off = 0; off < nj; off += chunk) {
                 const size_t cnt = std::min(chunk, nj - off);
@@ -1463,8 +1402,8 @@ void watermark_locked(ifb200_batch* b, const ifb200_watermark_desc* d, size_t n,
         }
         // 3. every composite of the chunk in one launch
         const uint32_t cta0 = wk.groups[c.g0].first, cta1 = c.g1 < ng ? wk.groups[c.g1].first : (uint32_t)wk.ctas();
-        watermark_composite_kernel<<<cta1 - cta0, ifb::kWmThreads, 0, st>>>(reinterpret_cast<const ifb::WmGroup*>(dbuf) + c.g0, c.g1 - c.g0,
-                                                                            reinterpret_cast<const ifb::WmJob*>(dbuf + o_jobs), b->tables, cta0);
+        watermark_composite_kernel<<<cta1 - cta0, ifb::kWmThreads, 0, st>>>(up.at<const ifb::WmGroup>(0) + c.g0, c.g1 - c.g0,
+                                                                            up.at<const ifb::WmJob>(1), b->tables, cta0);
         CUDA_OK(cudaGetLastError());
         b->launches++;
     }
@@ -1628,6 +1567,42 @@ void ensure(uint8_t*& p, size_t& cap, size_t need, cudaStream_t st) {
     cap = want;
 }
 
+// The body of every ifb200_batch_* operation: failures become a status, a null batch is rejected, and fn runs with the batch locked on
+// the caller's stream (IFB200_STREAM_OWN: the batch's own).
+template <class F>
+int with_batch(ifb200_batch* b, void* stream, char* err, size_t cap, F&& fn) {
+    return guarded(err, cap, [&] {
+        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
+        std::lock_guard<std::mutex> lk(b->mu);
+        fn(stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
+    });
+}
+
+// The drop-in calls on host buffers, after their argument checks: fn(batch, slot, stream) runs on slot 0 of the calling thread's
+// context, with its batch locked and its device current.
+template <class F>
+void on_host_slot(F&& fn) {
+    HostCtx& c = host_ctx();
+    std::lock_guard<std::mutex> lk(c.batch->mu);
+    DeviceScope dev_scope_(c.batch->device);
+    fn(c.batch, c.slot[0], c.slot[0].stream);
+}
+
+// A drop-in call that changes a host BGRA window in place: after the window's checks, the window goes to the slot's device image at
+// a 64-byte pitch, op(batch, device image, pitch, stream) runs on it, and the window comes back before the call returns.
+template <class F>
+void in_place_on_host(uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, F&& op) {
+    if (!bgra_window(px, w, h, stride)) return;
+    on_host_slot([&](ifb200_batch* b, HostSlot& sl, cudaStream_t st) {
+        const size_t pitch = ((size_t)w * 4 + 63) / 64 * 64;
+        ensure(sl.d_cv, sl.cap_cv, pitch * h, st);
+        CUDA_OK(cudaMemcpy2DAsync(sl.d_cv, pitch, px, stride, (size_t)w * 4, h, cudaMemcpyHostToDevice, st));
+        op(b, sl.d_cv, (uint32_t)pitch, st);
+        CUDA_OK(cudaMemcpy2DAsync(px, stride, sl.d_cv, pitch, (size_t)w * 4, h, cudaMemcpyDeviceToHost, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+    });
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -1774,111 +1749,60 @@ int ifb200_batch_create(int device, ifb200_batch** out, char* err, size_t cap) {
 }
 
 int ifb200_batch_enqueue(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n, void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b || (!descs && n)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch or descriptor array");
-        std::lock_guard<std::mutex> lk(b->mu);
-        enqueue_locked(b, descs, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { enqueue_locked(b, descs, n, st); });
 }
 
 int ifb200_batch_color_matrix(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, const float m[25],
                               void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        color_matrix_locked(b, dev_px, w, h, stride, m, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { color_matrix_locked(b, dev_px, w, h, stride, m, st); });
 }
 
 int ifb200_batch_apply_matte(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, const uint8_t matte_bgra[4],
                              int alpha_meaningful, void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        if (!alpha_meaningful) return;                       // blend.rs:10-13: nothing to do unless alpha is meaningful
-        std::lock_guard<std::mutex> lk(b->mu);
-        apply_matte_locked(b, dev_px, w, h, stride, matte_bgra, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) {
+        if (alpha_meaningful) apply_matte_locked(b, dev_px, w, h, stride, matte_bgra, st);   // blend.rs:10-13: nothing to do unless alpha is meaningful
     });
 }
 
 int ifb200_batch_transpose(ifb200_batch* b, const uint8_t* dev_from, uint32_t from_stride, uint32_t w, uint32_t h, uint8_t* dev_to,
                            uint32_t to_stride, void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        transpose_locked(b, dev_from, from_stride, w, h, dev_to, to_stride, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { transpose_locked(b, dev_from, from_stride, w, h, dev_to, to_stride, st); });
 }
 int ifb200_batch_flip_vertical(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        flip_locked(b, true, dev_px, w, h, stride, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { flip_locked(b, true, dev_px, w, h, stride, st); });
 }
 int ifb200_batch_flip_horizontal(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        flip_locked(b, false, dev_px, w, h, stride, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { flip_locked(b, false, dev_px, w, h, stride, st); });
 }
 
 int ifb200_batch_white_balance(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, float threshold, void* stream,
                                char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        white_balance_locked(b, dev_px, w, h, stride, threshold, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { white_balance_locked(b, dev_px, w, h, stride, threshold, st); });
 }
 
 int ifb200_batch_block_scale(ifb200_batch* b, const uint8_t* dev_in, uint32_t in_stride, uint32_t blocks_x, uint32_t blocks_y, uint8_t* dev_out,
                              uint32_t out_stride, int n, int srgb, void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        block_scale_locked(b, dev_in, in_stride, blocks_x, blocks_y, dev_out, out_stride, n, srgb, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { block_scale_locked(b, dev_in, in_stride, blocks_x, blocks_y, dev_out, out_stride, n, srgb, st); });
 }
 
 int ifb200_batch_round_corners(ifb200_batch* b, const ifb200_round_corners_desc* d, size_t n, void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        round_corners_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { round_corners_locked(b, d, n, st); });
 }
 
 int ifb200_batch_canvas(ifb200_batch* b, const ifb200_canvas_desc* d, size_t n, void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        canvas_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { canvas_locked(b, d, n, st); });
 }
 
 int ifb200_batch_orient(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        orient_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { orient_locked(b, d, n, st); });
 }
 
 int ifb200_batch_color_chain(ifb200_batch* b, const ifb200_color_desc* d, size_t n, void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        color_chain_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { color_chain_locked(b, d, n, st); });
 }
 
 int ifb200_batch_watermark(ifb200_batch* b, const ifb200_watermark_desc* d, size_t n, void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        watermark_locked(b, d, n, stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { watermark_locked(b, d, n, st); });
 }
 
 int ifb200_batch_sync(ifb200_batch* b, char* err, size_t cap) {
@@ -2027,20 +1951,10 @@ int ifb200_apply_matte_bgra8(uint8_t* px, uint32_t w, uint32_t h, uint32_t strid
                              char* err, size_t cap) {
     return guarded(err, cap, [&] {
         if (!px || !matte_bgra) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
-        if (!alpha_meaningful || w == 0 || h == 0) return;   // blend.rs:10-13
-        if (stride < w * 4ull || (stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "bad stride");
-        HostCtx& c = host_ctx();
-        ifb200_batch* b = c.batch;
-        std::lock_guard<std::mutex> lk(b->mu);
-        DeviceScope dev_scope_(b->device);
-        HostSlot& sl = c.slot[0];
-        cudaStream_t st = sl.stream;
-        const size_t pitch = ((size_t)w * 4 + 63) / 64 * 64;
-        ensure(sl.d_cv, sl.cap_cv, pitch * h, st);
-        CUDA_OK(cudaMemcpy2DAsync(sl.d_cv, pitch, px, stride, (size_t)w * 4, h, cudaMemcpyHostToDevice, st));
-        apply_matte_locked(b, sl.d_cv, w, h, (uint32_t)pitch, matte_bgra, st);
-        CUDA_OK(cudaMemcpy2DAsync(px, stride, sl.d_cv, pitch, (size_t)w * 4, h, cudaMemcpyDeviceToHost, st));
-        CUDA_OK(cudaStreamSynchronize(st));
+        if (!alpha_meaningful) return;                       // blend.rs:10-13
+        in_place_on_host(px, w, h, stride, [&](ifb200_batch* b, uint8_t* d, uint32_t pitch, cudaStream_t st) {
+            apply_matte_locked(b, d, w, h, pitch, matte_bgra, st);
+        });
     });
 }
 
@@ -2049,53 +1963,43 @@ int ifb200_apply_matte_bgra8(uint8_t* px, uint32_t w, uint32_t h, uint32_t strid
 int ifb200_round_corners_bgra8(const ifb200_round_corners_desc* d, char* err, size_t cap) {
     return guarded(err, cap, [&] {
         if (!d) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor");
-        round_corners_validate(*d);
+        const std::string why = ifb::round_corners_check(*d);
+        if (!why.empty()) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "%s", why.c_str());
         if (d->w == 0 || d->h == 0) return;
-        HostCtx& c = host_ctx();
-        ifb200_batch* b = c.batch;
-        std::lock_guard<std::mutex> lk(b->mu);
-        DeviceScope dev_scope_(b->device);
-        HostSlot& sl = c.slot[0];
-        cudaStream_t st = sl.stream;
-        const size_t pitch = ((size_t)d->w * 4 + 63) / 64 * 64;
-        ensure(sl.d_cv, sl.cap_cv, pitch * d->h, st);
-        const ifb::RcJob job = round_corners_job(*d, sl.d_cv, (uint32_t)pitch);
-        std::vector<ifb::RcRect> rects;
-        ifb::round_corners_cover(job, rects);
-        auto dev_at = [&](const ifb::RcRect& r) { return sl.d_cv + (size_t)r.y0 * pitch + (size_t)r.x0 * 4; };
-        auto host_at = [&](const ifb::RcRect& r) { return d->px + (size_t)r.y0 * d->stride + (size_t)r.x0 * 4; };
-        for (const auto& r : rects)
-            if (!r.fill_only) CUDA_OK(cudaMemcpy2DAsync(dev_at(r), pitch, host_at(r), d->stride, (size_t)r.w * 4, r.h, cudaMemcpyHostToDevice, st));
-        RcWork wk;
-        wk.add(job, rects);
-        round_corners_launch(b, wk, st);
-        for (const auto& r : rects)
-            CUDA_OK(cudaMemcpy2DAsync(host_at(r), d->stride, dev_at(r), pitch, (size_t)r.w * 4, r.h, cudaMemcpyDeviceToHost, st));
-        CUDA_OK(cudaStreamSynchronize(st));
+        on_host_slot([&](ifb200_batch* b, HostSlot& sl, cudaStream_t st) {
+            const size_t pitch = ((size_t)d->w * 4 + 63) / 64 * 64;
+            ensure(sl.d_cv, sl.cap_cv, pitch * d->h, st);
+            ifb200_round_corners_desc dd = *d;
+            dd.px = sl.d_cv; dd.stride = (uint32_t)pitch;
+            ifb::RcWork wk;
+            std::vector<ifb::RcRect> rects;
+            ifb::round_corners_plan(dd, wk, &rects);
+            auto dev_at = [&](const ifb::RcRect& r) { return sl.d_cv + (size_t)r.y0 * pitch + (size_t)r.x0 * 4; };
+            auto host_at = [&](const ifb::RcRect& r) { return d->px + (size_t)r.y0 * d->stride + (size_t)r.x0 * 4; };
+            for (const auto& r : rects)
+                if (!r.fill_only) CUDA_OK(cudaMemcpy2DAsync(dev_at(r), pitch, host_at(r), d->stride, (size_t)r.w * 4, r.h, cudaMemcpyHostToDevice, st));
+            round_corners_launch(b, wk, st);
+            for (const auto& r : rects)
+                CUDA_OK(cudaMemcpy2DAsync(host_at(r), d->stride, dev_at(r), pitch, (size_t)r.w * 4, r.h, cudaMemcpyDeviceToHost, st));
+            CUDA_OK(cudaStreamSynchronize(st));
+        });
     });
 }
 
 int ifb200_transpose_bgra8(const uint8_t* from, uint32_t from_stride, uint32_t w, uint32_t h, uint8_t* to, uint32_t to_stride,
                            char* err, size_t cap) {
     return guarded(err, cap, [&] {
-        if (!from || !to) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
-        if (w == 0 || h == 0) return;
-        if ((from_stride & 3) || (to_stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "strides must be multiples of 4 bytes");
-        if (from_stride < w * 4ull) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "from_stride(%u) < width(%u)", from_stride / 4, w);
-        if (to_stride < h * 4ull) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "to_stride(%u) < height(%u)", to_stride / 4, h);
-        HostCtx& c = host_ctx();
-        ifb200_batch* b = c.batch;
-        std::lock_guard<std::mutex> lk(b->mu);
-        DeviceScope dev_scope_(b->device);
-        HostSlot& sl = c.slot[0];
-        cudaStream_t st = sl.stream;
-        const size_t pin = ((size_t)w * 4 + 63) / 64 * 64, pout = ((size_t)h * 4 + 63) / 64 * 64;
-        ensure(sl.d_in, sl.cap_in, pin * h, st);
-        ensure(sl.d_cv, sl.cap_cv, pout * w, st);
-        CUDA_OK(cudaMemcpy2DAsync(sl.d_in, pin, from, from_stride, (size_t)w * 4, h, cudaMemcpyHostToDevice, st));
-        transpose_locked(b, sl.d_in, (uint32_t)pin, w, h, sl.d_cv, (uint32_t)pout, st);
-        CUDA_OK(cudaMemcpy2DAsync(to, to_stride, sl.d_cv, pout, (size_t)h * 4, w, cudaMemcpyDeviceToHost, st));
-        CUDA_OK(cudaStreamSynchronize(st));
+        if (!to) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
+        if (!bgra_window(from, w, h, from_stride) || !bgra_window(to, h, w, to_stride)) return;
+        on_host_slot([&](ifb200_batch* b, HostSlot& sl, cudaStream_t st) {
+            const size_t pin = ((size_t)w * 4 + 63) / 64 * 64, pout = ((size_t)h * 4 + 63) / 64 * 64;
+            ensure(sl.d_in, sl.cap_in, pin * h, st);
+            ensure(sl.d_cv, sl.cap_cv, pout * w, st);
+            CUDA_OK(cudaMemcpy2DAsync(sl.d_in, pin, from, from_stride, (size_t)w * 4, h, cudaMemcpyHostToDevice, st));
+            transpose_locked(b, sl.d_in, (uint32_t)pin, w, h, sl.d_cv, (uint32_t)pout, st);
+            CUDA_OK(cudaMemcpy2DAsync(to, to_stride, sl.d_cv, pout, (size_t)h * 4, w, cudaMemcpyDeviceToHost, st));
+            CUDA_OK(cudaStreamSynchronize(st));
+        });
     });
 }
 
@@ -2105,41 +2009,27 @@ int ifb200_detect_content_from_codes(const uint8_t* codes, uint32_t w, uint32_t 
 
 int ifb200_batch_detect_content(ifb200_batch* b, const uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, int alpha_meaningful,
                                 uint32_t threshold, uint32_t rect[4], void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        detect_content_locked(b, dev_px, w, h, stride, alpha_meaningful, threshold,
-                              stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream), rect);
-    });
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { detect_content_locked(b, dev_px, w, h, stride, alpha_meaningful, threshold, st, rect); });
 }
 
 int ifb200_batch_whitespace_codes(ifb200_batch* b, const uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, int alpha_meaningful,
                                   uint32_t threshold, uint8_t* dev_codes, void* stream, char* err, size_t cap) {
-    return guarded(err, cap, [&] {
-        if (!b) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null batch");
-        std::lock_guard<std::mutex> lk(b->mu);
-        DeviceScope dev_scope_(b->device);
-        whitespace_codes_locked(b, dev_px, w, h, stride, alpha_meaningful, threshold, dev_codes,
-                                stream == IFB200_STREAM_OWN ? b->own_stream : static_cast<cudaStream_t>(stream));
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) {
+        whitespace_codes_locked(b, dev_px, w, h, stride, alpha_meaningful, threshold, dev_codes, st);
     });
 }
 
 int ifb200_detect_content_bgra8(const uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, int alpha_meaningful, uint32_t threshold,
                                 uint32_t rect[4], char* err, size_t cap) {
     return guarded(err, cap, [&] {
-        if (!px || !rect) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
-        if (w == 0 || h == 0) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "empty bitmap");
-        if (stride < w * 4ull || (stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "bad stride");
-        HostCtx& c = host_ctx();
-        ifb200_batch* b = c.batch;
-        std::lock_guard<std::mutex> lk(b->mu);
-        DeviceScope dev_scope_(b->device);
-        HostSlot& sl = c.slot[0];
-        cudaStream_t st = sl.stream;
-        const size_t pitch = ((size_t)w * 4 + 63) / 64 * 64;
-        ensure(sl.d_cv, sl.cap_cv, pitch * h, st);
-        CUDA_OK(cudaMemcpy2DAsync(sl.d_cv, pitch, px, stride, (size_t)w * 4, h, cudaMemcpyHostToDevice, st));
-        detect_content_locked(b, sl.d_cv, w, h, (uint32_t)pitch, alpha_meaningful, threshold, st, rect);
+        if (!rect) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
+        if (!bgra_window(px, w, h, stride)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "empty bitmap");
+        on_host_slot([&](ifb200_batch* b, HostSlot& sl, cudaStream_t st) {
+            const size_t pitch = ((size_t)w * 4 + 63) / 64 * 64;
+            ensure(sl.d_cv, sl.cap_cv, pitch * h, st);
+            CUDA_OK(cudaMemcpy2DAsync(sl.d_cv, pitch, px, stride, (size_t)w * 4, h, cudaMemcpyHostToDevice, st));
+            detect_content_locked(b, sl.d_cv, w, h, (uint32_t)pitch, alpha_meaningful, threshold, st, rect);
+        });
     });
 }
 
@@ -2150,81 +2040,43 @@ int ifb200_block_scale_u8(const uint8_t* in, uint32_t in_stride, uint32_t blocks
         if (n < 1 || n > 7) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "block scalers exist for 1x1 .. 7x7 (got %d)", n);
         if (blocks_x == 0 || blocks_y == 0) return;
         if (in_stride < blocks_x * 8ull || out_stride < (uint64_t)blocks_x * (uint32_t)n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "stride smaller than a row of blocks");
-        HostCtx& c = host_ctx();
-        ifb200_batch* b = c.batch;
-        std::lock_guard<std::mutex> lk(b->mu);
-        DeviceScope dev_scope_(b->device);
-        HostSlot& sl = c.slot[0];
-        cudaStream_t st = sl.stream;
-        const size_t pin = ((size_t)blocks_x * 8 + 63) / 64 * 64, pout = ((size_t)blocks_x * n + 63) / 64 * 64;
-        ensure(sl.d_in, sl.cap_in, pin * blocks_y * 8, st);
-        ensure(sl.d_cv, sl.cap_cv, pout * blocks_y * n, st);
-        CUDA_OK(cudaMemcpy2DAsync(sl.d_in, pin, in, in_stride, (size_t)blocks_x * 8, (size_t)blocks_y * 8, cudaMemcpyHostToDevice, st));
-        block_scale_locked(b, sl.d_in, (uint32_t)pin, blocks_x, blocks_y, sl.d_cv, (uint32_t)pout, n, srgb, st);
-        CUDA_OK(cudaMemcpy2DAsync(out, out_stride, sl.d_cv, pout, (size_t)blocks_x * n, (size_t)blocks_y * n, cudaMemcpyDeviceToHost, st));
-        CUDA_OK(cudaStreamSynchronize(st));
+        on_host_slot([&](ifb200_batch* b, HostSlot& sl, cudaStream_t st) {
+            const size_t pin = ((size_t)blocks_x * 8 + 63) / 64 * 64, pout = ((size_t)blocks_x * n + 63) / 64 * 64;
+            ensure(sl.d_in, sl.cap_in, pin * blocks_y * 8, st);
+            ensure(sl.d_cv, sl.cap_cv, pout * blocks_y * n, st);
+            CUDA_OK(cudaMemcpy2DAsync(sl.d_in, pin, in, in_stride, (size_t)blocks_x * 8, (size_t)blocks_y * 8, cudaMemcpyHostToDevice, st));
+            block_scale_locked(b, sl.d_in, (uint32_t)pin, blocks_x, blocks_y, sl.d_cv, (uint32_t)pout, n, srgb, st);
+            CUDA_OK(cudaMemcpy2DAsync(out, out_stride, sl.d_cv, pout, (size_t)blocks_x * n, (size_t)blocks_y * n, cudaMemcpyDeviceToHost, st));
+            CUDA_OK(cudaStreamSynchronize(st));
+        });
     });
 }
 
 int ifb200_white_balance_srgb_bgra8(uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, float threshold, char* err, size_t cap) {
     return guarded(err, cap, [&] {
-        if (!px) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
-        if (w == 0 || h == 0) return;
-        if (stride < w * 4ull || (stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "bad stride");
-        HostCtx& c = host_ctx();
-        ifb200_batch* b = c.batch;
-        std::lock_guard<std::mutex> lk(b->mu);
-        DeviceScope dev_scope_(b->device);
-        HostSlot& sl = c.slot[0];
-        cudaStream_t st = sl.stream;
-        const size_t pitch = ((size_t)w * 4 + 63) / 64 * 64;
-        ensure(sl.d_cv, sl.cap_cv, pitch * h, st);
-        CUDA_OK(cudaMemcpy2DAsync(sl.d_cv, pitch, px, stride, (size_t)w * 4, h, cudaMemcpyHostToDevice, st));
-        white_balance_locked(b, sl.d_cv, w, h, (uint32_t)pitch, threshold, st);
-        CUDA_OK(cudaMemcpy2DAsync(px, stride, sl.d_cv, pitch, (size_t)w * 4, h, cudaMemcpyDeviceToHost, st));
-        CUDA_OK(cudaStreamSynchronize(st));
+        in_place_on_host(px, w, h, stride, [&](ifb200_batch* b, uint8_t* d, uint32_t pitch, cudaStream_t st) {
+            white_balance_locked(b, d, w, h, pitch, threshold, st);
+        });
     });
 }
 
-static int flip_host(bool vertical, uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, char* err, size_t cap) {
+int ifb200_flip_vertical_bgra8(uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, char* err, size_t cap) {
     return guarded(err, cap, [&] {
-        if (!px) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
-        if (w == 0 || h == 0) return;
-        if (stride < w * 4ull || (stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "bad stride");
-        HostCtx& c = host_ctx();
-        ifb200_batch* b = c.batch;
-        std::lock_guard<std::mutex> lk(b->mu);
-        DeviceScope dev_scope_(b->device);
-        HostSlot& sl = c.slot[0];
-        cudaStream_t st = sl.stream;
-        const size_t pitch = ((size_t)w * 4 + 63) / 64 * 64;
-        ensure(sl.d_cv, sl.cap_cv, pitch * h, st);
-        CUDA_OK(cudaMemcpy2DAsync(sl.d_cv, pitch, px, stride, (size_t)w * 4, h, cudaMemcpyHostToDevice, st));
-        flip_locked(b, vertical, sl.d_cv, w, h, (uint32_t)pitch, st);
-        CUDA_OK(cudaMemcpy2DAsync(px, stride, sl.d_cv, pitch, (size_t)w * 4, h, cudaMemcpyDeviceToHost, st));
-        CUDA_OK(cudaStreamSynchronize(st));
+        in_place_on_host(px, w, h, stride, [&](ifb200_batch* b, uint8_t* d, uint32_t pitch, cudaStream_t st) { flip_locked(b, true, d, w, h, pitch, st); });
     });
 }
-int ifb200_flip_vertical_bgra8(uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, char* err, size_t cap) { return flip_host(true, px, w, h, stride, err, cap); }
-int ifb200_flip_horizontal_bgra8(uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, char* err, size_t cap) { return flip_host(false, px, w, h, stride, err, cap); }
+int ifb200_flip_horizontal_bgra8(uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, char* err, size_t cap) {
+    return guarded(err, cap, [&] {
+        in_place_on_host(px, w, h, stride, [&](ifb200_batch* b, uint8_t* d, uint32_t pitch, cudaStream_t st) { flip_locked(b, false, d, w, h, pitch, st); });
+    });
+}
 
 int ifb200_color_matrix_bgra8(uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, const float m[25], char* err, size_t cap) {
     return guarded(err, cap, [&] {
-        if (!px || !m) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
-        if (w == 0 || h == 0) return;
-        if (stride < w * 4ull || (stride & 3)) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "bad stride");
-        HostCtx& c = host_ctx();
-        ifb200_batch* b = c.batch;
-        std::lock_guard<std::mutex> lk(b->mu);
-        DeviceScope dev_scope_(b->device);
-        HostSlot& sl = c.slot[0];
-        cudaStream_t st = sl.stream;
-        const size_t pitch = ((size_t)w * 4 + 63) / 64 * 64;
-        ensure(sl.d_cv, sl.cap_cv, pitch * h, st);
-        CUDA_OK(cudaMemcpy2DAsync(sl.d_cv, pitch, px, stride, (size_t)w * 4, h, cudaMemcpyHostToDevice, st));
-        color_matrix_locked(b, sl.d_cv, w, h, (uint32_t)pitch, m, st);
-        CUDA_OK(cudaMemcpy2DAsync(px, stride, sl.d_cv, pitch, (size_t)w * 4, h, cudaMemcpyDeviceToHost, st));
-        CUDA_OK(cudaStreamSynchronize(st));
+        if (!m) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
+        in_place_on_host(px, w, h, stride, [&](ifb200_batch* b, uint8_t* d, uint32_t pitch, cudaStream_t st) {
+            color_matrix_locked(b, d, w, h, pitch, m, st);
+        });
     });
 }
 

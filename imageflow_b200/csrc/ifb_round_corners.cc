@@ -37,15 +37,16 @@ void plan_custom(const float r[4], uint32_t w, uint32_t h, QuadrantInfo q[4]) {
     q[3] = {left_half_width, top_half_height, right_half_width, bottom_half_height, r[3], (float)w - r[3], (float)h - r[3], false, false};
 }
 
-}  // namespace
-
-bool round_corners_plan(int mode, const float radius[4], uint32_t w, uint32_t h, RcJob* job) {
-    // get_radius (rounded_corners.rs:5-33).  Its Custom array is [tl, tr, bl, br]; radius[] is in field order [tl, tr, br, bl].
+// The job of a valid, non-empty descriptor.  get_radius (rounded_corners.rs:5-33): its Custom array is [tl, tr, bl, br]; d.radius
+// is in the field order of RoundCornersMode::*Custom [tl, tr, br, bl].
+RcJob plan_job(const ifb200_round_corners_desc& d) {
+    const uint32_t w = d.w, h = d.h;
+    const float* radius = d.radius;
     const float smallest = (float)std::min(w, h);
     auto pct = [&](float p) { return smallest * clampf(p, 0.0f, 100.0f) / 200.0f; };
     auto pix = [&](float p) { return clampf(p, 0.0f, smallest / 2.0f); };
     QuadrantInfo q[4];
-    switch (mode) {
+    switch (d.mode) {
     case IFB200_CORNERS_PERCENTAGE: { const float v = pct(radius[0]); const float r[4] = {v, v, v, v}; plan_custom(r, w, h, q); break; }
     case IFB200_CORNERS_PIXELS: { const float v = pix(radius[0]); const float r[4] = {v, v, v, v}; plan_custom(r, w, h, q); break; }
     case IFB200_CORNERS_PERCENTAGE_CUSTOM: {
@@ -56,7 +57,7 @@ bool round_corners_plan(int mode, const float radius[4], uint32_t w, uint32_t h,
         const float r[4] = {pix(radius[0]), pix(radius[1]), pix(radius[3]), pix(radius[2])};
         plan_custom(r, w, h, q); break;
     }
-    case IFB200_CORNERS_CIRCLE: {                                // :46-64: the quadrants of the centred square, moved
+    default: {                                                   // IFB200_CORNERS_CIRCLE, :46-64: the quadrants of the centred square, moved
         const uint32_t s = std::min(w, h);
         const uint32_t off_x = (uint32_t)(std::max<int64_t>((int64_t)w - (int64_t)h, 0) / 2);
         const uint32_t off_y = (uint32_t)(std::max<int64_t>((int64_t)h - (int64_t)w, 0) / 2);
@@ -66,16 +67,18 @@ bool round_corners_plan(int mode, const float radius[4], uint32_t w, uint32_t h,
         for (auto& e : q) { e.x += off_x; e.y += off_y; e.cx += (float)off_x; e.cy += (float)off_y; }
         break;
     }
-    default: return false;
     }
 
     const float volumetric_offset = 0.56419f;                 // :200-202
-    job->w = w; job->h = h;
-    job->top_rows = q[0].y;                                  // :209-212 (q[0].y > 0 only for CIRCLE on a tall frame)
-    job->bottom_from = std::min(h, q[2].y + q[2].height);    // :213-216
+    RcJob job{};
+    job.px = d.px; job.stride = d.stride;
+    job.matte = (uint32_t)d.matte_bgra[0] | ((uint32_t)d.matte_bgra[1] << 8) | ((uint32_t)d.matte_bgra[2] << 16) | ((uint32_t)d.matte_bgra[3] << 24);
+    job.w = w; job.h = h;
+    job.top_rows = q[0].y;                                   // :209-212 (q[0].y > 0 only for CIRCLE on a tall frame)
+    job.bottom_from = std::min(h, q[2].y + q[2].height);     // :213-216
     for (int i = 0; i < 4; ++i) {
         const QuadrantInfo& a = q[i];
-        RcQuad& o = job->q[i];
+        RcQuad& o = job.q[i];
         const uint32_t bottom = a.y + a.height, right = a.x + a.width;
         const uint64_t radius_ceil = as_usize(std::ceil(a.radius));
         // :218-227; the clamps only matter where the reference would index out of bounds
@@ -93,7 +96,33 @@ bool round_corners_plan(int mode, const float radius[4], uint32_t w, uint32_t h,
         o.clear_to = a.is_left ? a.x : w;
         o.is_left = a.is_left ? 1u : 0u;
     }
-    return true;
+    return job;
+}
+
+}  // namespace
+
+std::string round_corners_check(const ifb200_round_corners_desc& d) {
+    if (d.mode < IFB200_CORNERS_PERCENTAGE || d.mode > IFB200_CORNERS_PIXELS_CUSTOM) return "unknown corners mode " + std::to_string(d.mode);
+    if (d.w == 0 || d.h == 0) return "";
+    if (!d.px) return "null bitmap pointer";
+    if (d.stride < d.w * 4ull || (d.stride & 3)) return "stride smaller than a BGRA row or not a multiple of 4";
+    if ((uint64_t)d.w * d.h > 0xffffffffull) return "bitmap too large";
+    return "";
+}
+
+void round_corners_plan(const ifb200_round_corners_desc& d, RcWork& wk, std::vector<RcRect>* rects) {
+    if (d.w == 0 || d.h == 0) return;
+    const RcJob job = plan_job(d);
+    std::vector<RcRect> cover;
+    round_corners_cover(job, cover);
+    const uint32_t j = (uint32_t)wk.jobs.size();
+    wk.jobs.push_back(job);
+    for (const RcRect& r : cover) {
+        const uint64_t area = (uint64_t)r.w * r.h;
+        for (uint64_t f = 0; f < area; f += kRcTilePixels)
+            wk.tiles.push_back({j, r.x0, r.y0, r.w, (uint32_t)f, (uint32_t)std::min<uint64_t>(kRcTilePixels, area - f)});
+    }
+    if (rects) rects->insert(rects->end(), cover.begin(), cover.end());
 }
 
 void round_corners_cover(const RcJob& job, std::vector<RcRect>& out) {

@@ -1,9 +1,13 @@
 // ifb_round_corners.h -- host planner of flow_bitmap_bgra_clear_around_rounded_corners (graphics/rounded_corners.rs:1-346).
-// Product code, plain C++ without CUDA calls (tests/cpu_emu links it unchanged): get_radius and plan_quadrants in f32 with the
-// reference's operation order, and a cover of every pixel the op can touch as disjoint rectangles.
+// Product code, plain C++ without CUDA calls (tests/cpu_emu links it unchanged): validation of each descriptor, get_radius and
+// plan_quadrants in f32 with the reference's operation order, a cover of every pixel the op can touch as disjoint rectangles, and
+// the cut of that cover into CTA tiles of one flat launch.
 #pragma once
 #include <cstdint>
+#include <string>
 #include <vector>
+
+#include "../../include/ifb200.h"
 
 namespace ifb {
 
@@ -37,9 +41,17 @@ struct RcTile { uint32_t job, x0, y0, rw, first, count; };
 // (so its old contents are never read).
 struct RcRect { uint32_t x0, y0, w, h; bool fill_only; };
 
-// radius[] in the field order of RoundCornersMode::*Custom (top_left, top_right, bottom_right, bottom_left); mode as
-// ifb200_corners_mode.  Returns false for an unknown mode.  w and h must be > 0.
-bool round_corners_plan(int mode, const float radius[4], uint32_t w, uint32_t h, RcJob* job);
+struct RcWork {
+    std::vector<RcJob> jobs; std::vector<RcTile> tiles;
+};
+
+// Empty when d is a valid descriptor, else why it is not (the call then fails with IFB200_ERR_INVALID_ARGUMENT).  Degenerate radii
+// are not errors: the plan gives them the reference's meaning.
+std::string round_corners_check(const ifb200_round_corners_desc& d);
+
+// Appends the job of a valid descriptor on its bitmap (d.px, d.stride) and the tiles of its cover to `wk`, and the cover itself to
+// `*rects` when given.  Nothing for an empty window.
+void round_corners_plan(const ifb200_round_corners_desc& d, RcWork& wk, std::vector<RcRect>* rects = nullptr);
 
 // Disjoint rectangles that together cover every pixel any step of `job` can write.  Each row's cover is a prefix [0, L) and a
 // suffix [R, w) of the row (every step works from the left or the right edge); inside a corner's square the cover also holds the

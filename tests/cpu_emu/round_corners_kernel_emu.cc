@@ -5,6 +5,8 @@
 #include <cmath>
 #include <cstddef>
 #include <cstdint>
+#include <cstdio>
+#include <string>
 #include <vector>
 
 #include "../../include/ifb200.h"
@@ -38,42 +40,31 @@ namespace ifbk {
 #include "../../imageflow_b200/csrc/ifb_round_corners_kernel.cuh"
 }  // namespace ifbk
 
-// One launch over descs[0..n) as ifb200_batch_round_corners makes it (ifb_engine.cu: round_corners_job, RcWork, round_corners_launch).
-// loads / stores receive the byte address of every pixel access, in order (capacity cap each; *n_loads / *n_stores = the counts).
-// Returns the number of CTAs launched, or -1 for a bad mode.
+// One call of ifb200_batch_round_corners over d[0..n) as the engine makes it (ifb_engine.cu round_corners_locked): every descriptor
+// checked first, then planned, then one launch.  loads / stores receive the byte address of every pixel access, in order (capacity
+// cap each; *n_loads / *n_stores = the counts).  Returns the number of CTAs launched, or -1 when a descriptor is rejected (err = why).
 extern "C" long emu_round_corners(const ifb200_round_corners_desc* d, size_t n, const float* t_lin, const uint8_t* lut16k,
-                                  uint64_t* loads, uint64_t* stores, size_t cap, size_t* n_loads, size_t* n_stores) {
-    std::vector<ifb::RcJob> jobs;
-    std::vector<ifb::RcTile> tiles;
-    std::vector<ifb::RcRect> rects;
+                                  uint64_t* loads, uint64_t* stores, size_t cap, size_t* n_loads, size_t* n_stores, char* err, size_t err_cap) {
     for (size_t i = 0; i < n; ++i) {
-        if (d[i].w == 0 || d[i].h == 0) continue;
-        ifb::RcJob job{};
-        if (!ifb::round_corners_plan(d[i].mode, d[i].radius, d[i].w, d[i].h, &job)) return -1;
-        job.px = d[i].px; job.stride = d[i].stride;
-        job.matte = (uint32_t)d[i].matte_bgra[0] | ((uint32_t)d[i].matte_bgra[1] << 8) | ((uint32_t)d[i].matte_bgra[2] << 16) |
-                    ((uint32_t)d[i].matte_bgra[3] << 24);
-        rects.clear();
-        ifb::round_corners_cover(job, rects);
-        const uint32_t j = (uint32_t)jobs.size();
-        jobs.push_back(job);
-        for (const auto& r : rects) {
-            const uint64_t area = (uint64_t)r.w * r.h;
-            for (uint64_t f = 0; f < area; f += ifb::kRcTilePixels)
-                tiles.push_back({j, r.x0, r.y0, r.w, (uint32_t)f, (uint32_t)(area - f < ifb::kRcTilePixels ? area - f : ifb::kRcTilePixels)});
+        const std::string why = ifb::round_corners_check(d[i]);
+        if (!why.empty()) {
+            snprintf(err, err_cap, "round corners job %zu: %s", i, why.c_str());
+            return -1;
         }
     }
+    ifb::RcWork wk;
+    for (size_t i = 0; i < n; ++i) ifb::round_corners_plan(d[i], wk);
     emu::loads.clear(); emu::stores.clear();
     const ifbk::Tables tb{t_lin, nullptr, lut16k};
-    for (unsigned b = 0; b < tiles.size(); ++b) {
+    for (unsigned b = 0; b < wk.tiles.size(); ++b) {
         emu::blockIdx = {b, 0, 0};
         for (unsigned t = 0; t < ifb::kRcThreads; ++t) {
             emu::threadIdx = {t, 0, 0};
-            ifbk::round_corners_kernel(jobs.data(), tiles.data(), tb);
+            ifbk::round_corners_kernel(wk.jobs.data(), wk.tiles.data(), tb);
         }
     }
     *n_loads = emu::loads.size(); *n_stores = emu::stores.size();
     for (size_t i = 0; i < emu::loads.size() && i < cap; ++i) loads[i] = emu::loads[i];
     for (size_t i = 0; i < emu::stores.size() && i < cap; ++i) stores[i] = emu::stores[i];
-    return (long)tiles.size();
+    return (long)wk.tiles.size();
 }

@@ -36,7 +36,7 @@ def load(so):
     L = C.CDLL(so)
     L.emu_round_corners.restype = C.c_long
     L.emu_round_corners.argtypes = [C.POINTER(RoundCornersDesc), C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
-                                    C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+                                    C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.c_char_p, C.c_size_t]
     return L
 
 
@@ -87,9 +87,11 @@ def run(so, n_launches=600, seed=1):
         cap = sum(w * h for w, h, *_ in jobs) * 2 + 16
         loads, stores = np.zeros(cap, np.uint64), np.zeros(cap, np.uint64)
         nl, ns = C.c_size_t(), C.c_size_t()
+        err = C.create_string_buffer(256)
         ctas = L.emu_round_corners(descs, len(jobs), t_lin.ctypes.data, lut.ctypes.data, loads.ctypes.data, stores.ctypes.data, cap,
-                                   C.byref(nl), C.byref(ns))
-        assert ctas >= 0 and nl.value <= cap and ns.value <= cap
+                                   C.byref(nl), C.byref(ns), err, 256)
+        assert ctas >= 0, err.value.decode()
+        assert nl.value <= cap and ns.value <= cap
         st, ld = stores[:ns.value].tolist(), loads[:nl.value].tolist()
         assert len(set(st)) == len(st), ("a pixel stored twice", jobs)
         assert set(st) == want_stores, ("stored set differs from the oracle's touch mask", jobs)
