@@ -4,6 +4,8 @@
 #include <algorithm>
 #include <cstdio>
 
+#include "ifb_prepare.h"
+
 namespace ifb {
 namespace {
 
@@ -84,7 +86,8 @@ void plan_copy(const ifb200_canvas_desc& d, bool am, bool in_am, uint32_t fx, ui
 
 }  // namespace
 
-std::string canvas_check(const ifb200_canvas_desc& d) {
+std::string canvas_check(const ifb200_canvas_desc& d, int* code) {
+    if (code) *code = IFB200_ERR_INVALID_ARGUMENT;
     if (d.op < IFB200_CANVAS_FILL_RECT || d.op > IFB200_CANVAS_NORMALIZE_ALPHA) return fmt("unknown canvas op %llu", (unsigned)d.op);
     std::string e = check_window("canvas", d.px, d.w, d.h, d.stride);
     if (!e.empty()) return e;
@@ -133,6 +136,13 @@ void canvas_plan(const ifb200_canvas_desc& d, CvWork& wk) {
     }
     default: break;
     }
+}
+
+std::string canvas_prepare(const ifb200_canvas_desc* d, size_t n, CvWork& wk, int* code) {
+    const std::string why = check_each("canvas", d, n, canvas_check, code);
+    if (why.empty())
+        for (size_t i = 0; i < n; ++i) canvas_plan(d[i], wk);
+    return why;
 }
 
 }  // namespace ifb

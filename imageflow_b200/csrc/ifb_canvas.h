@@ -34,11 +34,15 @@ struct CvWork {
     std::vector<CvItem> items; std::vector<CvTile> tiles;
 };
 
-// Empty when d is a valid descriptor, else why it is not (the call then fails with IFB200_ERR_INVALID_ARGUMENT).
-std::string canvas_check(const ifb200_canvas_desc& d);
+// Empty when d is a valid descriptor, else why it is not; *code, when given, = IFB200_ERR_INVALID_ARGUMENT (its only status).
+std::string canvas_check(const ifb200_canvas_desc& d, int* code = nullptr);
 
 // Appends the work items of a valid descriptor and their tiles to `wk`: disjoint rectangles, so that every pixel the op writes is
 // written by one thread, once.  Nothing for a job that writes no pixel.
 void canvas_plan(const ifb200_canvas_desc& d, CvWork& wk);
+
+// Checks every descriptor of one call, then plans all of them into wk.  Empty on success; else "canvas job i: <why>" for the first
+// rejected descriptor, with *code = its status, and nothing planned.
+std::string canvas_prepare(const ifb200_canvas_desc* d, size_t n, CvWork& wk, int* code);
 
 }  // namespace ifb

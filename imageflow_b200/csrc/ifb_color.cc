@@ -5,6 +5,7 @@
 #include <algorithm>
 
 #include "ifb_orient.h"   // groups_per_row
+#include "ifb_prepare.h"
 
 namespace ifb {
 namespace {
@@ -160,6 +161,13 @@ void color_plan(const ifb200_color_desc& d, ClWork& wk) {
     }
     if (j.nseg == 0) return;                           // nothing but EnableTransparency on Bgra32: no pixel changes
     add_job(wk, j);
+}
+
+std::string color_prepare(const ifb200_color_desc* d, size_t n, ClWork& wk, int* code) {
+    const std::string why = check_each("color", d, n, color_check, code);
+    if (why.empty())
+        for (size_t i = 0; i < n; ++i) color_plan(d[i], wk);
+    return why;
 }
 
 }  // namespace ifb

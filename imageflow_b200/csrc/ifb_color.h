@@ -60,6 +60,10 @@ std::string color_check(const ifb200_color_desc& d, int* code);
 // Appends the job of a valid descriptor (nothing for a job with no pixels or no steps).
 void color_plan(const ifb200_color_desc& d, ClWork& wk);
 
+// Checks every descriptor of one call, then plans all of them into wk.  Empty on success; else "color job i: <why>" for the first
+// rejected descriptor, with *code = its status, and nothing planned.
+std::string color_prepare(const ifb200_color_desc* d, size_t n, ClWork& wk, int* code);
+
 // color.rs:101-108 uchar_clamp_ff on the host
 uint8_t color_clamp(float v);
 

@@ -1205,12 +1205,10 @@ void round_corners_launch(ifb200_batch* b, const ifb::RcWork& wk, cudaStream_t s
 // enqueued, then all jobs run in ONE launch.
 void round_corners_locked(ifb200_batch* b, const ifb200_round_corners_desc* d, size_t n, cudaStream_t st) {
     if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
-    for (size_t i = 0; i < n; ++i) {
-        const std::string why = ifb::round_corners_check(d[i]);
-        if (!why.empty()) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "round corners job %zu: %s", i, why.c_str());
-    }
     ifb::RcWork wk;
-    for (size_t i = 0; i < n; ++i) ifb::round_corners_plan(d[i], wk);
+    int code = 0;
+    const std::string why = ifb::round_corners_prepare(d, n, wk, &code);
+    if (!why.empty()) IFB_THROW(code, "%s", why.c_str());
     round_corners_launch(b, wk, st);
 }
 
@@ -1218,12 +1216,10 @@ void round_corners_locked(ifb200_batch* b, const ifb200_round_corners_desc* d, s
 // then all jobs run in ONE launch (none when no job writes a pixel).
 void canvas_locked(ifb200_batch* b, const ifb200_canvas_desc* d, size_t n, cudaStream_t st) {
     if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
-    for (size_t i = 0; i < n; ++i) {
-        const std::string why = ifb::canvas_check(d[i]);
-        if (!why.empty()) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "canvas job %zu: %s", i, why.c_str());
-    }
     ifb::CvWork wk;
-    for (size_t i = 0; i < n; ++i) ifb::canvas_plan(d[i], wk);
+    int code = 0;
+    const std::string why = ifb::canvas_prepare(d, n, wk, &code);
+    if (!why.empty()) IFB_THROW(code, "%s", why.c_str());
     if (wk.tiles.empty()) return;
     if (wk.tiles.size() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
     DeviceScope dev_scope_(b->device);
@@ -1237,12 +1233,10 @@ void canvas_locked(ifb200_batch* b, const ifb200_canvas_desc* d, size_t n, cudaS
 // all jobs run in ONE launch (none when no job writes a pixel).  The upload is the items and their first CTAs, O(jobs).
 void orient_locked(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, cudaStream_t st) {
     if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
-    for (size_t i = 0; i < n; ++i) {
-        const std::string why = ifb::orient_check(d[i]);
-        if (!why.empty()) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "orient job %zu: %s", i, why.c_str());
-    }
     ifb::OrWork wk;
-    for (size_t i = 0; i < n; ++i) ifb::orient_plan(d[i], wk);
+    int code = 0;
+    const std::string why = ifb::orient_prepare(d, n, wk, &code);
+    if (!why.empty()) IFB_THROW(code, "%s", why.c_str());
     if (wk.items.empty()) return;
     if (wk.ctas() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
     DeviceScope dev_scope_(b->device);
@@ -1257,13 +1251,10 @@ void orient_locked(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, cudaS
 // job white-balances (histograms into zeroed counters, byte maps into the jobs' kClWb tables, apply); none when no job writes a pixel.
 void color_chain_locked(ifb200_batch* b, const ifb200_color_desc* d, size_t n, cudaStream_t st) {
     if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
-    for (size_t i = 0; i < n; ++i) {
-        int code = 0;
-        const std::string why = ifb::color_check(d[i], &code);
-        if (!why.empty()) IFB_THROW(code, "color job %zu: %s", i, why.c_str());
-    }
     ifb::ClWork wk;
-    for (size_t i = 0; i < n; ++i) ifb::color_plan(d[i], wk);
+    int code = 0;
+    const std::string why = ifb::color_prepare(d, n, wk, &code);
+    if (!why.empty()) IFB_THROW(code, "%s", why.c_str());
     if (wk.jobs.empty()) return;
     if (wk.ctas() > 0x7fffffffu || wk.wb_ctas() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
     DeviceScope dev_scope_(b->device);
@@ -1299,14 +1290,11 @@ constexpr size_t kWmScratchBytes = (size_t)1 << 30;
 void watermark_locked(ifb200_batch* b, const ifb200_watermark_desc* d, size_t n, cudaStream_t st) {
     if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
     Tick tk_all(b->prof.enqueue);
-    for (size_t i = 0; i < n; ++i) {
-        int code = 0;
-        const std::string why = ifb::watermark_check(d[i], &code);
-        if (!why.empty()) IFB_THROW(code, "watermark job %zu: %s", i, why.c_str());
-    }
     host_tables();
     ifb::WmWork wk;
-    ifb::watermark_plan(d, n, g_t_lin_host, g_t_srgb_host, wk);
+    int code = 0;
+    const std::string why = ifb::watermark_prepare(d, n, g_t_lin_host, g_t_srgb_host, wk, &code);
+    if (!why.empty()) IFB_THROW(code, "%s", why.c_str());
     if (wk.groups.empty()) return;
     if (wk.ctas() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
     DeviceScope dev_scope_(b->device);
@@ -1963,8 +1951,9 @@ int ifb200_apply_matte_bgra8(uint8_t* px, uint32_t w, uint32_t h, uint32_t strid
 int ifb200_round_corners_bgra8(const ifb200_round_corners_desc* d, char* err, size_t cap) {
     return guarded(err, cap, [&] {
         if (!d) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor");
-        const std::string why = ifb::round_corners_check(*d);
-        if (!why.empty()) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "%s", why.c_str());
+        int code = 0;
+        const std::string why = ifb::round_corners_check(*d, &code);
+        if (!why.empty()) IFB_THROW(code, "%s", why.c_str());
         if (d->w == 0 || d->h == 0) return;
         on_host_slot([&](ifb200_batch* b, HostSlot& sl, cudaStream_t st) {
             const size_t pitch = ((size_t)d->w * 4 + 63) / 64 * 64;

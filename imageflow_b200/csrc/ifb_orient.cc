@@ -3,6 +3,8 @@
 
 #include <algorithm>
 
+#include "ifb_prepare.h"
+
 namespace ifb {
 namespace {
 
@@ -46,7 +48,8 @@ uint32_t groups_per_row(const uint8_t* row0, uint32_t stride, uint32_t xlim) {
 
 int32_t orient_flag(int32_t o) { return o >= 2 && o <= 8 ? o : 1; }
 
-std::string orient_check(const ifb200_orient_desc& d) {
+std::string orient_check(const ifb200_orient_desc& d, int* code) {
+    if (code) *code = IFB200_ERR_INVALID_ARGUMENT;
     if (d.in_w == 0 || d.in_h == 0) return "";
     if ((uint64_t)d.in_w * d.in_h > 0xffffffffull) return "window too large";
     const int32_t o = orient_flag(d.orientation);
@@ -95,6 +98,13 @@ void orient_plan(const ifb200_orient_desc& d, OrWork& wk) {
         add_groups(wk, it, 0, h / 2, w);
         if (h & 1) add_groups(wk, it, h / 2, 1, w / 2);   // the middle row swaps within itself; its middle pixel stays
     }
+}
+
+std::string orient_prepare(const ifb200_orient_desc* d, size_t n, OrWork& wk, int* code) {
+    const std::string why = check_each("orient", d, n, orient_check, code);
+    if (why.empty())
+        for (size_t i = 0; i < n; ++i) orient_plan(d[i], wk);
+    return why;
 }
 
 }  // namespace ifb

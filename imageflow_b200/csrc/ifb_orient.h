@@ -46,11 +46,15 @@ uint32_t groups_per_row(const uint8_t* row0, uint32_t stride, uint32_t xlim);
 // The orientation a flag stands for: 2..8 as they are, every other value 1 (the identity).
 int32_t orient_flag(int32_t orientation);
 
-// Empty when d is a valid descriptor, else why it is not (the call then fails with IFB200_ERR_INVALID_ARGUMENT).
-std::string orient_check(const ifb200_orient_desc& d);
+// Empty when d is a valid descriptor, else why it is not; *code, when given, = IFB200_ERR_INVALID_ARGUMENT (its only status).
+std::string orient_check(const ifb200_orient_desc& d, int* code = nullptr);
 
 // Appends the work items of a valid descriptor (none for a job that writes no pixel) and keeps wk.first a prefix sum with a
 // trailing total.
 void orient_plan(const ifb200_orient_desc& d, OrWork& wk);
+
+// Checks every descriptor of one call, then plans all of them into wk.  Empty on success; else "orient job i: <why>" for the first
+// rejected descriptor, with *code = its status, and nothing planned.
+std::string orient_prepare(const ifb200_orient_desc* d, size_t n, OrWork& wk, int* code);
 
 }  // namespace ifb

@@ -8,6 +8,7 @@
 #include <cmath>
 
 #include "../../include/ifb200.h"
+#include "ifb_prepare.h"
 
 namespace ifb {
 namespace {
@@ -101,7 +102,8 @@ RcJob plan_job(const ifb200_round_corners_desc& d) {
 
 }  // namespace
 
-std::string round_corners_check(const ifb200_round_corners_desc& d) {
+std::string round_corners_check(const ifb200_round_corners_desc& d, int* code) {
+    if (code) *code = IFB200_ERR_INVALID_ARGUMENT;
     if (d.mode < IFB200_CORNERS_PERCENTAGE || d.mode > IFB200_CORNERS_PIXELS_CUSTOM) return "unknown corners mode " + std::to_string(d.mode);
     if (d.w == 0 || d.h == 0) return "";
     if (!d.px) return "null bitmap pointer";
@@ -123,6 +125,13 @@ void round_corners_plan(const ifb200_round_corners_desc& d, RcWork& wk, std::vec
             wk.tiles.push_back({j, r.x0, r.y0, r.w, (uint32_t)f, (uint32_t)std::min<uint64_t>(kRcTilePixels, area - f)});
     }
     if (rects) rects->insert(rects->end(), cover.begin(), cover.end());
+}
+
+std::string round_corners_prepare(const ifb200_round_corners_desc* d, size_t n, RcWork& wk, int* code) {
+    const std::string why = check_each("round corners", d, n, round_corners_check, code);
+    if (why.empty())
+        for (size_t i = 0; i < n; ++i) round_corners_plan(d[i], wk);
+    return why;
 }
 
 void round_corners_cover(const RcJob& job, std::vector<RcRect>& out) {

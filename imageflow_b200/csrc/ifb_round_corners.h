@@ -45,13 +45,17 @@ struct RcWork {
     std::vector<RcJob> jobs; std::vector<RcTile> tiles;
 };
 
-// Empty when d is a valid descriptor, else why it is not (the call then fails with IFB200_ERR_INVALID_ARGUMENT).  Degenerate radii
-// are not errors: the plan gives them the reference's meaning.
-std::string round_corners_check(const ifb200_round_corners_desc& d);
+// Empty when d is a valid descriptor, else why it is not; *code, when given, = IFB200_ERR_INVALID_ARGUMENT (its only status).
+// Degenerate radii are not errors: the plan gives them the reference's meaning.
+std::string round_corners_check(const ifb200_round_corners_desc& d, int* code = nullptr);
 
 // Appends the job of a valid descriptor on its bitmap (d.px, d.stride) and the tiles of its cover to `wk`, and the cover itself to
 // `*rects` when given.  Nothing for an empty window.
 void round_corners_plan(const ifb200_round_corners_desc& d, RcWork& wk, std::vector<RcRect>* rects = nullptr);
+
+// Checks every descriptor of one call, then plans all of them into wk.  Empty on success; else "round corners job i: <why>" for the
+// first rejected descriptor, with *code = its status, and nothing planned.
+std::string round_corners_prepare(const ifb200_round_corners_desc* d, size_t n, RcWork& wk, int* code);
 
 // Disjoint rectangles that together cover every pixel any step of `job` can write.  Each row's cover is a prefix [0, L) and a
 // suffix [R, w) of the row (every step works from the left or the right edge); inside a corner's square the cover also holds the

@@ -6,6 +6,7 @@
 #include <unordered_map>
 
 #include "ifb_orient.h"   // groups_per_row
+#include "ifb_prepare.h"
 
 namespace ifb {
 namespace {
@@ -128,6 +129,12 @@ void watermark_plan(const ifb200_watermark_desc* d, size_t n, const float* t_lin
             wk.jobs.push_back(j);
         }
     }
+}
+
+std::string watermark_prepare(const ifb200_watermark_desc* d, size_t n, const float* t_lin, const float* t_srgb, WmWork& wk, int* code) {
+    const std::string why = check_each("watermark", d, n, watermark_check, code);
+    if (why.empty()) watermark_plan(d, n, t_lin, t_srgb, wk);
+    return why;
 }
 
 }  // namespace ifb

@@ -55,4 +55,8 @@ bool watermark_opacity(float opacity, float* applied);
 // Plans d[0..n) (all checked): groups, jobs and CTAs.  t_lin / t_srgb: byte_to_float tables (for the matte, as make_job).
 void watermark_plan(const ifb200_watermark_desc* d, size_t n, const float* t_lin, const float* t_srgb, WmWork& wk);
 
+// Checks every descriptor of one call, then plans all of them into wk.  Empty on success; else "watermark job i: <why>" for the first
+// rejected descriptor, with *code = its status, and nothing planned.
+std::string watermark_prepare(const ifb200_watermark_desc* d, size_t n, const float* t_lin, const float* t_srgb, WmWork& wk, int* code);
+
 }  // namespace ifb

@@ -4,11 +4,47 @@ of a kernel can be checked without a GPU.  Nothing in the product imports this p
 import ctypes as C
 import os
 import subprocess
+import sys
 
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+ROOT = os.path.dirname(os.path.dirname(HERE))
+CSRC = os.path.join(ROOT, "imageflow_b200", "csrc")
 u32, f32 = C.c_uint32, C.c_float
+# every emulator library is built with the same flags: the kernels' arithmetic is never contracted into fused multiply-adds it
+# does not spell out (-ffp-contract=off), and the threaded emulators need std::barrier and std::thread (C++20, -pthread)
+CXXFLAGS = ["-O1", "-g", "-std=c++20", "-pthread", "-shared", "-fPIC", "-ffp-contract=off", "-Wall", "-Wno-unknown-pragmas",
+            "-Wno-implicit-fallthrough"]
+ASAN_FLAGS = ["-fsanitize=address", "-fno-omit-frame-pointer"]
+
+
+def _libasan() -> str:
+    """the path of g++'s libasan; skips the calling test when there is none (an instrumented build could not link)"""
+    import pytest
+    asan = subprocess.run(["g++", "-print-file-name=libasan.so"], capture_output=True, text=True).stdout.strip()
+    if not os.path.isabs(asan) or not os.path.exists(asan):
+        pytest.skip("libasan not available")
+    return asan
+
+
+def build(out_dir: str, emu_source: str, *product_sources: str, sanitize: bool = False) -> str:
+    """g++ of tests/cpu_emu/<emu_source> with the product's host sources imageflow_b200/csrc/<product_sources> it links, into a
+    library in out_dir (instrumented by AddressSanitizer when `sanitize`).  Returns its path."""
+    if sanitize:
+        _libasan()
+    name = os.path.splitext(emu_source)[0] + ("_asan" if sanitize else "")
+    so = os.path.join(out_dir, f"lib{name}.so")
+    cmd = ["g++", *CXXFLAGS, *(ASAN_FLAGS if sanitize else []), "-o", so, os.path.join(HERE, emu_source)]
+    subprocess.run(cmd + [os.path.join(CSRC, s) for s in product_sources], check=True)
+    return so
+
+
+def run_under_asan(module: str, so: str, n: int, timeout: int = 1200) -> subprocess.CompletedProcess:
+    """python -m tests.cpu_emu.<module> <so> <n> with libasan preloaded (the test is skipped when g++ has no libasan)"""
+    env = dict(os.environ, LD_PRELOAD=_libasan(), ASAN_OPTIONS="detect_leaks=0:verify_asan_link_order=0", PYTHONPATH=ROOT)
+    return subprocess.run([sys.executable, "-m", f"tests.cpu_emu.{module}", so, str(n)], capture_output=True, text=True, cwd=ROOT,
+                          env=env, timeout=timeout)
 
 
 class JobDev(C.Structure):                          # imageflow_b200/csrc/ifb_types.cuh
@@ -16,13 +52,34 @@ class JobDev(C.Structure):                          # imageflow_b200/csrc/ifb_ty
                 ("matte", f32 * 4), ("cm", f32 * 20)]
 
 
-def build_tile2(out_dir: str, sanitize: bool = False) -> str:
-    so = os.path.join(out_dir, "libtile2_emu_asan.so" if sanitize else "libtile2_emu.so")
-    cmd = ["g++", "-O1", "-g", "-std=c++20", "-pthread", "-shared", "-fPIC", "-ffp-contract=off"]
-    if sanitize:
-        cmd += ["-fsanitize=address", "-fno-omit-frame-pointer"]
-    subprocess.run(cmd + ["-o", so, os.path.join(HERE, "tile2_kernel_emu.cc")], check=True)
-    return so
+def transfer_tables(ifb):
+    """(t_lin, t_srgb, lut16k): the library's byte-to-float tables of both working spaces and its linear-to-sRGB table"""
+    t_lin, t_srgb, lut = np.zeros(256, np.float32), np.zeros(256, np.float32), np.zeros(16384, np.uint8)
+    f32p, u8p = C.POINTER(C.c_float), C.POINTER(C.c_uint8)
+    ifb.lib().ifb200_byte_to_float_table(1, t_lin.ctypes.data_as(f32p)); ifb.lib().ifb200_byte_to_float_table(0, t_srgb.ctypes.data_as(f32p))
+    ifb.lib().ifb200_linear_to_srgb_table(lut.ctypes.data_as(u8p))
+    return t_lin, t_srgb, lut
+
+
+def set_job_store(j, t_lin, t_srgb, *, linear, alpha_meaningful, compose, matte, color_matrix):
+    """JobDev's flags, premultiplied matte and transposed colour matrix, as make_job (ifb_engine.cu) sets them"""
+    j.flags = (1 if linear else 0) | (2 if alpha_meaningful else 0) | (compose << 2)
+    if compose == 2 and alpha_meaningful:
+        T = t_lin if linear else t_srgb
+        ma = np.float32(matte[3]) * np.float32(1.0 / 255.0)
+        for c in range(3):
+            j.matte[c] = float(np.float32(T[matte[c]]) * ma)
+        j.matte[3] = float(ma)
+    if color_matrix is not None:
+        m = np.ascontiguousarray(color_matrix, np.float32).reshape(25)
+        j.flags |= 16
+        for c in range(4):
+            for k in range(4):
+                j.cm[c * 5 + k] = float(m[k * 5 + c])
+            j.cm[c * 5 + 4] = float(np.float32(m[20 + c]) * np.float32(255.0))
+        cm = np.array(list(j.cm), np.float32)
+        if all(cm[15 + k] == (1.0 if k == 3 else 0.0) for k in range(5)) and all(cm[c * 5 + 3] == 0 and cm[c * 5 + 4] == 0 for c in range(3)):
+            j.flags |= 32
 
 
 def csr(ws):
@@ -67,10 +124,7 @@ def run_tile2(lib, ifb, inp, canvas, *, x=0, y=0, w=None, h=None, filter=14, lin
             for j in range(int(hl[xx]), int(hr[xx]) + 1):
                 t_hw[xx, j - int(hl[xx])] = hw[int(ho[xx]) + j - int(hl[xx])]
     plan = np.array([iw, ih, w, h, 64, th, tiles_x, tiles_y, max_ic, max_ir, h4], np.int32)
-    t_lin, t_srgb, lut = (np.zeros(256, np.float32), np.zeros(256, np.float32), np.zeros(16384, np.uint8))
-    f32p, u8p = C.POINTER(C.c_float), C.POINTER(C.c_uint8)
-    ifb.lib().ifb200_byte_to_float_table(1, t_lin.ctypes.data_as(f32p)); ifb.lib().ifb200_byte_to_float_table(0, t_srgb.ctypes.data_as(f32p))
-    ifb.lib().ifb200_linear_to_srgb_table(lut.ctypes.data_as(u8p))
+    t_lin, t_srgb, lut = transfer_tables(ifb)
     assert L.emu_tile2_sizeof_jobdev() == C.sizeof(JobDev)
     inp = np.ascontiguousarray(inp)
     outs = [np.ascontiguousarray(canvas.copy()) for _ in range(jobs_repeat)]
@@ -79,23 +133,7 @@ def run_tile2(lib, ifb, inp, canvas, *, x=0, y=0, w=None, h=None, filter=14, lin
     for j, o in zip(jobs, outs):
         j.in_ = inp.ctypes.data; j.out = o.ctypes.data + y * o.strides[0] + x * 4
         j.in_stride, j.out_stride = inp.strides[0], o.strides[0]
-        j.flags = (1 if linear else 0) | (2 if alpha_meaningful else 0) | (compose << 2)
-        if compose == 2 and alpha_meaningful:
-            T = t_lin if linear else t_srgb
-            ma = np.float32(matte[3]) * np.float32(1.0 / 255.0)
-            for c in range(3):
-                j.matte[c] = float(np.float32(T[matte[c]]) * ma)
-            j.matte[3] = float(ma)
-        if color_matrix is not None:
-            m = np.ascontiguousarray(color_matrix, np.float32).reshape(25)
-            j.flags |= 16
-            for c in range(4):
-                for k in range(4):
-                    j.cm[c * 5 + k] = float(m[k * 5 + c])
-                j.cm[c * 5 + 4] = float(np.float32(m[20 + c]) * np.float32(255.0))
-            cm = np.array(list(j.cm), np.float32)
-            if all(cm[15 + k] == (1.0 if k == 3 else 0.0) for k in range(5)) and all(cm[c * 5 + 3] == 0 and cm[c * 5 + 4] == 0 for c in range(3)):
-                j.flags |= 32
+        set_job_store(j, t_lin, t_srgb, linear=linear, alpha_meaningful=alpha_meaningful, compose=compose, matte=matte, color_matrix=color_matrix)
     p = lambda a, t: a.ctypes.data_as(C.POINTER(t))
     rc = L.emu_tile2_launch(ch, int(linear), compose, int(color_matrix is not None), grid, C.cast(jobs, C.c_void_p), jobs_repeat,
                             p(t_lin, C.c_float), p(t_srgb, C.c_float), p(lut, C.c_uint8),
@@ -119,15 +157,6 @@ class HvPlanInfo(C.Structure):                      # include/ifb200.h ifb200_hv
     _fields_ = [("ok", C.c_int32), ("av", C.c_int32), ("n_strips", C.c_int32), ("n_bands", C.c_int32), ("cap_px", C.c_int32), ("avp", C.c_int32),
                 ("o_strips", C.c_uint64), ("o_hw", C.c_uint64), ("o_hdone", C.c_uint64), ("o_vw", C.c_uint64), ("o_vdone", C.c_uint64),
                 ("o_bands", C.c_uint64), ("total", C.c_uint64)]
-
-
-def build_hv(out_dir: str, sanitize: bool = False) -> str:
-    so = os.path.join(out_dir, "libhv_emu_asan.so" if sanitize else "libhv_emu.so")
-    cmd = ["g++", "-O1", "-g", "-std=c++20", "-pthread", "-shared", "-fPIC", "-ffp-contract=off", "-Wno-implicit-fallthrough"]
-    if sanitize:
-        cmd += ["-fsanitize=address", "-fno-omit-frame-pointer"]
-    subprocess.run(cmd + ["-o", so, os.path.join(HERE, "hv_kernel_emu.cc")], check=True)
-    return so
 
 
 def load_hv(so):
@@ -168,10 +197,7 @@ def run_hv(lib, ifb, inp, canvas, *, x=0, y=0, w=None, h=None, filter=2, sharpen
     info, blob = hv_plan(ifb, iw, ih, w, h, filter, sharpen, strip_cols, n_bands, alpha_meaningful)      # n_bands = band PAIRS
     if blob is None:
         return None
-    t_lin, t_srgb, lut = (np.zeros(256, np.float32), np.zeros(256, np.float32), np.zeros(16384, np.uint8))
-    f32p, u8p = C.POINTER(C.c_float), C.POINTER(C.c_uint8)
-    ifb.lib().ifb200_byte_to_float_table(1, t_lin.ctypes.data_as(f32p)); ifb.lib().ifb200_byte_to_float_table(0, t_srgb.ctypes.data_as(f32p))
-    ifb.lib().ifb200_linear_to_srgb_table(lut.ctypes.data_as(u8p))
+    t_lin, t_srgb, lut = transfer_tables(ifb)
     assert lib.emu_hv_sizeof_jobdev() == C.sizeof(JobDev)
     # the input as a window of a wider, 16-byte aligned bitmap
     pitch = ((iw + in_xoff) * 4 + 63) // 64 * 64
@@ -185,20 +211,7 @@ def run_hv(lib, ifb, inp, canvas, *, x=0, y=0, w=None, h=None, filter=2, sharpen
     for j, o in zip(jobs, outs):
         j.in_ = wide.ctypes.data + in_xoff * 4; j.out = o.ctypes.data + y * o.strides[0] + x * 4
         j.in_stride, j.out_stride, j.in_xoff = pitch, o.strides[0], in_xoff
-        j.flags = (1 if linear else 0) | (2 if alpha_meaningful else 0) | (compose << 2)
-        if compose == 2 and alpha_meaningful:
-            T = t_lin if linear else t_srgb
-            ma = np.float32(matte[3]) * np.float32(1.0 / 255.0)
-            for c in range(3):
-                j.matte[c] = float(np.float32(T[matte[c]]) * ma)
-            j.matte[3] = float(ma)
-        if color_matrix is not None:
-            m = np.ascontiguousarray(color_matrix, np.float32).reshape(25)
-            j.flags |= 16
-            for c in range(4):
-                for k in range(4):
-                    j.cm[c * 5 + k] = float(m[k * 5 + c])
-                j.cm[c * 5 + 4] = float(np.float32(m[20 + c]) * np.float32(255.0))
+        set_job_store(j, t_lin, t_srgb, linear=linear, alpha_meaningful=alpha_meaningful, compose=compose, matte=matte, color_matrix=color_matrix)
     in_ptrs = (C.c_void_p * jobs_repeat)(*[wide.ctypes.data] * jobs_repeat)
     in_whs = np.array([iw + in_xoff, ih, pitch] * jobs_repeat, np.uint32)
     offs = np.array([info.o_strips, info.o_hw, info.o_hdone, info.o_vw, info.o_vdone, info.o_bands, info.total], np.uint64)

@@ -5,12 +5,10 @@
 // effects of segment p (shared and global stores, atomics, recorded loads) take place; the other segments run dry.  So each
 // segment sees the complete effects of the one before it, as on the GPU.  The address of each 4-byte pixel that a global pixel load
 // or store touches is recorded (a 16-byte access records its four pixels).
-#include <algorithm>
-#include <cmath>
+#include "cuda_emu.h"
+
 #include <cstddef>
-#include <cstdint>
 #include <cstdio>
-#include <cstring>
 #include <string>
 #include <vector>
 
@@ -18,8 +16,6 @@
 #include "../../imageflow_b200/csrc/ifb_color.h"
 
 namespace emu {
-struct Idx { unsigned x, y, z; };
-static Idx threadIdx, blockIdx;
 static int pass, seg;
 static std::vector<uint64_t> loads, stores;
 static bool live() { return seg == pass; }
@@ -44,23 +40,8 @@ template <class T> static T add(T* p, T v) {
     return o;
 }
 }  // namespace emu
-#define __global__
-#define __device__
-#define __forceinline__ inline
-#define __restrict__
-#define __launch_bounds__(...)
 #define __shared__ static
 #define __syncthreads() do { if (emu::seg == emu::pass) return; ++emu::seg; } while (0)
-using emu::blockIdx;
-using emu::threadIdx;
-struct uint4 { uint32_t x, y, z, w; };
-static inline uint4 make_uint4(uint32_t x, uint32_t y, uint32_t z, uint32_t w) { return {x, y, z, w}; }
-static inline float __fmul_rn(float a, float b) { return a * b; }
-static inline float __fadd_rn(float a, float b) { return a + b; }
-static inline double __ddiv_rn(double a, double b) { return a / b; }
-static inline double __dmul_rn(double a, double b) { return a * b; }
-using std::max;
-using std::min;
 #define IFB_CL_LOAD4(p) emu::load(p)
 #define IFB_CL_STORE4(p, v) emu::store(p, (uint32_t)(v))
 #define IFB_CL_LOAD16(p) emu::load(p)
@@ -88,8 +69,8 @@ void run_ctas(void (*kernel)(ifbk::ClDev), const ifbk::ClDev& a, uint64_t ctas, 
 }
 }  // namespace
 
-// One call of ifb200_batch_color_chain over d[0..n) as the engine makes it (ifb_engine.cu color_chain_locked): every descriptor
-// checked first, then planned, then the histogram, maps and apply launches (the first two only when a job white-balances).
+// One call of ifb200_batch_color_chain over d[0..n) as the engine makes it: color_prepare, which color_chain_locked (ifb_engine.cu)
+// calls too, then the histogram, maps and apply launches (the first two only when a job white-balances).
 // loads / stores receive the address of every pixel access, in order (capacity cap each; *n_loads / *n_stores = the counts);
 // hist receives the 768 counters of each white balance as the histogram launch left them (capacity hist_cap counters; *n_wb = the
 // white balances).  *launches = the kernel launches.  Returns the CTAs launched, or -(ifb200_status) when a descriptor is rejected
@@ -101,16 +82,13 @@ extern "C" long emu_color(const ifb200_color_desc* d, size_t n, uint64_t* loads,
                           size_t* n_stores, uint64_t* hist, size_t hist_cap, size_t* n_wb, int* launches, char* err, size_t err_cap,
                           int sabotage) {
     *launches = 0; *n_wb = 0; *n_loads = 0; *n_stores = 0;
-    for (size_t i = 0; i < n; ++i) {
-        int code = 0;
-        const std::string why = ifb::color_check(d[i], &code);
-        if (!why.empty()) {
-            snprintf(err, err_cap, "color job %zu: %s", i, why.c_str());
-            return -code;
-        }
-    }
     ifb::ClWork wk;
-    for (size_t i = 0; i < n; ++i) ifb::color_plan(d[i], wk);
+    int code = 0;
+    const std::string why = ifb::color_prepare(d, n, wk, &code);
+    if (!why.empty()) {
+        snprintf(err, err_cap, "%s", why.c_str());
+        return -code;
+    }
     if (wk.jobs.empty()) return 0;
     if (sabotage == 1 && wk.jobs.size() > 1) --wk.first[1];
     if (sabotage == 2) ++wk.jobs[0].tab0;
@@ -143,12 +121,9 @@ extern "C" long emu_color(const ifb200_color_desc* d, size_t n, uint64_t* loads,
 extern "C" long emu_color_plan(const ifb200_color_desc* d, size_t n, size_t* bytes, size_t* n_jobs, uint32_t* kinds, size_t kinds_cap,
                                size_t* n_segs) {
     ifb::ClWork wk;
-    for (size_t i = 0; i < n; ++i) {
-        int code = 0;
-        if (!ifb::color_check(d[i], &code).empty()) return -1;
-        ifb::color_plan(d[i], wk);
-    }
-    *bytes = wk.bytes(); *n_jobs = wk.jobs.size(); *n_segs = wk.segs.size();
+    int code = 0;
+    if (!ifb::color_prepare(d, n, wk, &code).empty()) return -1;
+    *bytes =wk.bytes(); *n_jobs = wk.jobs.size(); *n_segs = wk.segs.size();
     for (size_t i = 0; i < wk.segs.size() && i < kinds_cap; ++i) kinds[i] = wk.segs[i].kind;
     return (long)wk.ctas();
 }
@@ -156,11 +131,8 @@ extern "C" long emu_color_plan(const ifb200_color_desc* d, size_t n, size_t* byt
 // The tables of a plan (for the planner tests): every table of every job in order, 1024 bytes each (capacity cap bytes).
 extern "C" long emu_color_tables(const ifb200_color_desc* d, size_t n, uint8_t* out, size_t cap) {
     ifb::ClWork wk;
-    for (size_t i = 0; i < n; ++i) {
-        int code = 0;
-        if (!ifb::color_check(d[i], &code).empty()) return -1;
-        ifb::color_plan(d[i], wk);
-    }
+    int code = 0;
+    if (!ifb::color_prepare(d, n, wk, &code).empty()) return -1;
     memcpy(out, wk.tables.data(), std::min(cap, wk.tables.size()));
     return (long)wk.tables.size();
 }

@@ -5,24 +5,19 @@
 // zero fill outside the bitmap.  CTAs of the grid run one after the other (they only share the per-strip work counters).
 // Built with -ffp-contract=off; with -fsanitize=address a run is also a memory check of the kernel.
 // TEST INFRASTRUCTURE: nothing in the product calls this; the GPU remains the place where the kernel is run and timed.
-#include <algorithm>
+#include "cuda_emu.h"
+
 #include <atomic>
 #include <barrier>
-#include <cmath>
 #include <cstddef>
-#include <cstdint>
 #include <cstdio>
 #include <cstdlib>
-#include <cstring>
 #include <memory>
 #include <thread>
 #include <vector>
 
 #define IFB_HV_EMU 1
 namespace emu {
-struct Idx { unsigned x, y, z; };
-static thread_local Idx threadIdx;
-static Idx blockIdx, gridDim;
 static unsigned char* smem;
 static size_t smem_bytes;
 static uint32_t win_base;                                  // fake shared-window address of smem[0]
@@ -36,29 +31,6 @@ static inline unsigned char* at(uint32_t a, size_t n) {
     return smem + off;
 }
 }  // namespace emu
-using emu::blockIdx;
-using emu::gridDim;
-#define threadIdx emu::threadIdx
-#define __global__
-#define __device__
-#define __host__
-#define __forceinline__ inline
-#define __restrict__
-#define __launch_bounds__(...)
-using std::max;
-using std::min;
-struct alignas(8) float2 { float x, y; };
-struct alignas(16) float4 { float x, y, z, w; };
-struct alignas(16) uint4 { uint32_t x, y, z, w; };
-static inline float2 make_float2(float x, float y) { return float2{x, y}; }
-static inline float4 make_float4(float x, float y, float z, float w) { return float4{x, y, z, w}; }
-static inline float __fmaf_rn(float a, float b, float c) { return std::fmaf(a, b, c); }
-static inline float __fmul_rn(float a, float b) { return a * b; }
-static inline float __fadd_rn(float a, float b) { return a + b; }
-static inline float __fsub_rn(float a, float b) { return a - b; }
-static inline float __fdiv_rn(float a, float b) { return a / b; }
-static inline float __uint2float_rn(unsigned v) { return (float)v; }
-static inline int __ffs(int v) { return __builtin_ffs(v); }
 
 struct EmuTmap { const uint8_t* base; uint32_t w, h, stride; unsigned char pad[128 - 8 - 12]; };   // same size as a CUtensorMap
 
@@ -168,7 +140,6 @@ using HvTmapEmu = EmuTmap;
 #include "../../imageflow_b200/csrc/ifb_hv_kernel.cuh"
 #undef HvTmap
 }  // namespace ifbk
-#undef threadIdx
 
 using namespace ifbk;
 static_assert(sizeof(EmuTmap) == 128 && sizeof(HvTmapDecl) == 128, "descriptor size");

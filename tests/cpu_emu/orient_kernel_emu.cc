@@ -5,11 +5,10 @@
 // barrier (global stores are dropped, no access is recorded); pass 1 runs through and records the address of each 4-byte pixel
 // every global load and store touches (a 16-byte access records its four pixels).  Shared-memory indices outside the
 // kOrTileOx x 32 tile are counted.
-#include <algorithm>
+#include "cuda_emu.h"
+
 #include <cstddef>
-#include <cstdint>
 #include <cstdio>
-#include <cstring>
 #include <string>
 #include <vector>
 
@@ -17,8 +16,6 @@
 #include "../../imageflow_b200/csrc/ifb_orient.h"
 
 namespace emu {
-struct Idx { unsigned x, y, z; };
-static Idx threadIdx, blockIdx;
 static int pass;
 static long bad_smem;
 static std::vector<uint64_t> loads, stores;
@@ -43,19 +40,8 @@ static uint32_t& smem(uint32_t (*t)[33], uint32_t r, uint32_t c) {
     return t[r][c];
 }
 }  // namespace emu
-#define __global__
-#define __device__
-#define __forceinline__ inline
-#define __restrict__
-#define __launch_bounds__(...)
 #define __shared__ static
 #define __syncthreads() do { if (emu::pass == 0) return; } while (0)
-using emu::blockIdx;
-using emu::threadIdx;
-struct uint4 { uint32_t x, y, z, w; };
-static inline uint4 make_uint4(uint32_t x, uint32_t y, uint32_t z, uint32_t w) { return {x, y, z, w}; }
-using std::max;
-using std::min;
 #define IFB_OR_LOAD4(p) emu::load(p)
 #define IFB_OR_STORE4(p, v) emu::store(p, (uint32_t)(v))
 #define IFB_OR_LOAD16(p) emu::load(p)
@@ -66,23 +52,21 @@ namespace ifbk {
 #include "../../imageflow_b200/csrc/ifb_orient_kernel.cuh"
 }  // namespace ifbk
 
-// One call of ifb200_batch_orient over d[0..n) as the engine makes it (ifb_engine.cu orient_locked): every descriptor checked
-// first, then planned, then one launch.  loads / stores receive the address of every pixel access, in order (capacity cap each;
+// One call of ifb200_batch_orient over d[0..n) as the engine makes it: orient_prepare, which orient_locked (ifb_engine.cu) calls too,
+// then one launch.  loads / stores receive the address of every pixel access, in order (capacity cap each;
 // *n_loads / *n_stores = the counts), *bad_smem the shared-memory indices outside the tile.  Returns the number of CTAs launched,
 // or -1 when a descriptor is rejected (err = why).  *n_items = the work items planned.
 // sabotage != 0 corrupts the plan before the launch, to show that the checks of the tests catch it: 1 toggles the x reversal of
 // the first item (a neighbouring orientation), 2 moves the first item's output one pixel to the right, 3 drops the last CTA.
 extern "C" long emu_orient(const ifb200_orient_desc* d, size_t n, uint64_t* loads, uint64_t* stores, size_t cap, size_t* n_loads,
                            size_t* n_stores, long* bad_smem, size_t* n_items, char* err, size_t err_cap, int sabotage) {
-    for (size_t i = 0; i < n; ++i) {
-        const std::string why = ifb::orient_check(d[i]);
-        if (!why.empty()) {
-            snprintf(err, err_cap, "orient job %zu: %s", i, why.c_str());
-            return -1;
-        }
-    }
     ifb::OrWork wk;
-    for (size_t i = 0; i < n; ++i) ifb::orient_plan(d[i], wk);
+    int code = 0;
+    const std::string why = ifb::orient_prepare(d, n, wk, &code);
+    if (!why.empty()) {
+        snprintf(err, err_cap, "%s", why.c_str());
+        return -1;
+    }
     *n_items = wk.items.size();
     uint64_t ctas = wk.ctas();
     if (sabotage == 1 && !wk.items.empty()) wk.items.front().flags ^= ifb::kOrFx;
@@ -106,10 +90,8 @@ extern "C" long emu_orient(const ifb200_orient_desc* d, size_t n, uint64_t* load
 // The plan alone: the number of work items and CTAs of one call (-1 when a descriptor is rejected).
 extern "C" long emu_orient_plan(const ifb200_orient_desc* d, size_t n, size_t* n_items) {
     ifb::OrWork wk;
-    for (size_t i = 0; i < n; ++i) {
-        if (!ifb::orient_check(d[i]).empty()) return -1;
-        ifb::orient_plan(d[i], wk);
-    }
+    int code = 0;
+    if (!ifb::orient_prepare(d, n, wk, &code).empty()) return -1;
     *n_items = wk.items.size();
     return (long)wk.ctas();
 }

@@ -2,9 +2,9 @@
 // sequential emulation of the few CUDA built-ins it uses, with the product's host planner (ifb_round_corners.cc, linked as it is).
 // TEST INFRASTRUCTURE: nothing in the product calls it.  The kernel has no barrier and no shared memory, so the threads of a CTA
 // simply run one after the other.  Every pixel load and store goes through IFB_RC_LOAD / IFB_RC_STORE, which record the address.
-#include <cmath>
+#include "cuda_emu.h"
+
 #include <cstddef>
-#include <cstdint>
 #include <cstdio>
 #include <string>
 #include <vector>
@@ -13,24 +13,8 @@
 #include "../../imageflow_b200/csrc/ifb_round_corners.h"
 
 namespace emu {
-struct Idx { unsigned x, y, z; };
-static Idx threadIdx, blockIdx;
 static std::vector<uint64_t> loads, stores;
 }  // namespace emu
-#define __global__
-#define __device__
-#define __forceinline__ inline
-#define __restrict__
-#define __launch_bounds__(...)
-using emu::blockIdx;
-using emu::threadIdx;
-template <class T> static inline T __ldg(const T* p) { return *p; }
-static inline float __fmul_rn(float a, float b) { return a * b; }
-static inline float __fadd_rn(float a, float b) { return a + b; }
-static inline float __fsub_rn(float a, float b) { return a - b; }
-static inline float __fdiv_rn(float a, float b) { return a / b; }
-static inline float __fsqrt_rn(float a) { return std::sqrt(a); }
-static inline float __uint2float_rn(unsigned v) { return (float)v; }
 #define IFB_RC_LOAD(p) (emu::loads.push_back((uint64_t)(uintptr_t)(p)), *(p))
 #define IFB_RC_STORE(p, v) (emu::stores.push_back((uint64_t)(uintptr_t)(p)), *(p) = (v))
 
@@ -40,20 +24,18 @@ namespace ifbk {
 #include "../../imageflow_b200/csrc/ifb_round_corners_kernel.cuh"
 }  // namespace ifbk
 
-// One call of ifb200_batch_round_corners over d[0..n) as the engine makes it (ifb_engine.cu round_corners_locked): every descriptor
-// checked first, then planned, then one launch.  loads / stores receive the byte address of every pixel access, in order (capacity
+// One call of ifb200_batch_round_corners over d[0..n) as the engine makes it: round_corners_prepare, which round_corners_locked
+// (ifb_engine.cu) calls too, then one launch.  loads / stores receive the byte address of every pixel access, in order (capacity
 // cap each; *n_loads / *n_stores = the counts).  Returns the number of CTAs launched, or -1 when a descriptor is rejected (err = why).
 extern "C" long emu_round_corners(const ifb200_round_corners_desc* d, size_t n, const float* t_lin, const uint8_t* lut16k,
                                   uint64_t* loads, uint64_t* stores, size_t cap, size_t* n_loads, size_t* n_stores, char* err, size_t err_cap) {
-    for (size_t i = 0; i < n; ++i) {
-        const std::string why = ifb::round_corners_check(d[i]);
-        if (!why.empty()) {
-            snprintf(err, err_cap, "round corners job %zu: %s", i, why.c_str());
-            return -1;
-        }
-    }
     ifb::RcWork wk;
-    for (size_t i = 0; i < n; ++i) ifb::round_corners_plan(d[i], wk);
+    int code = 0;
+    const std::string why = ifb::round_corners_prepare(d, n, wk, &code);
+    if (!why.empty()) {
+        snprintf(err, err_cap, "%s", why.c_str());
+        return -1;
+    }
     emu::loads.clear(); emu::stores.clear();
     const ifbk::Tables tb{t_lin, nullptr, lut16k};
     for (unsigned b = 0; b < wk.tiles.size(); ++b) {

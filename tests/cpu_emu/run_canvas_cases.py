@@ -10,8 +10,6 @@ so that rows start at every phase modulo 16 bytes and a copy's source and destin
   - the pixels stored are exactly the pixels the oracle writes;
   - the pixels loaded are copy sources or pixels normalised in place, each loaded at most once."""
 import ctypes as C
-import os
-import subprocess
 import sys
 
 import numpy as np
@@ -19,19 +17,8 @@ import numpy as np
 from imageflow_b200._lib import CanvasDesc
 from tests import canvas_oracle as co
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(os.path.dirname(HERE))
-CSRC = os.path.join(ROOT, "imageflow_b200", "csrc")
+SOURCES = ("canvas_kernel_emu.cc", "ifb_canvas.cc")          # of tests.cpu_emu.build
 FILL, COPY, EXPAND, NORMALIZE = range(4)
-
-
-def build(out_dir: str, sanitize: bool = False) -> str:
-    so = os.path.join(out_dir, "libcanvas_emu_asan.so" if sanitize else "libcanvas_emu.so")
-    cmd = ["g++", "-O1", "-g", "-std=c++17", "-shared", "-fPIC", "-Wall"]
-    if sanitize:
-        cmd += ["-fsanitize=address", "-fno-omit-frame-pointer"]
-    subprocess.run(cmd + ["-o", so, os.path.join(HERE, "canvas_kernel_emu.cc"), os.path.join(CSRC, "ifb_canvas.cc")], check=True)
-    return so
 
 
 def load(so):

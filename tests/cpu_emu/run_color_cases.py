@@ -12,8 +12,6 @@ EnableTransparency on Bgr32 and Bgra32 windows, and white balance.  Per launch:
   - every load is in a window, each pixel loaded once per pass (twice for a job that white-balances);
   - the counters of each white balance equal the oracle's histograms of the frame as the chain leaves it before the white balance."""
 import ctypes as C
-import os
-import subprocess
 import sys
 
 import numpy as np
@@ -22,21 +20,9 @@ from imageflow_b200._lib import ColorDesc, ColorStep
 from tests import color_oracle as co
 from tests.cpu_emu.run_orient_cases import window_in
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(os.path.dirname(HERE))
-CSRC = os.path.join(ROOT, "imageflow_b200", "csrc")
+SOURCES = ("color_kernel_emu.cc", "ifb_color.cc", "ifb_orient.cc")          # of tests.cpu_emu.build
 SIZES = [(1, 1), (1, 7), (7, 1), (5, 3), (31, 5), (33, 9), (64, 3), (65, 2), (2, 65), (129, 17)]
 MATRIX, ENABLE_TRANSPARENCY, WHITE_BALANCE = 0, 1, 2
-
-
-def build(out_dir: str, sanitize: bool = False) -> str:
-    so = os.path.join(out_dir, "libcolor_emu_asan.so" if sanitize else "libcolor_emu.so")
-    cmd = ["g++", "-O1", "-g", "-std=c++17", "-shared", "-fPIC", "-Wall", "-Wno-unknown-pragmas", "-ffp-contract=off"]
-    if sanitize:
-        cmd += ["-fsanitize=address", "-fno-omit-frame-pointer"]
-    subprocess.run(cmd + ["-o", so, os.path.join(HERE, "color_kernel_emu.cc"), os.path.join(CSRC, "ifb_color.cc"),
-                          os.path.join(CSRC, "ifb_orient.cc")], check=True)
-    return so
 
 
 def load(so):

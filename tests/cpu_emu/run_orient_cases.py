@@ -11,8 +11,6 @@ bases fall at every 4-byte phase modulo 16.  Per launch:
   - no pixel is loaded twice, and every load is in the input window (in place: among the pixels the flip moves);
   - no shared-memory index falls outside the tile."""
 import ctypes as C
-import os
-import subprocess
 import sys
 
 import numpy as np
@@ -20,19 +18,8 @@ import numpy as np
 from imageflow_b200._lib import OrientDesc
 from tests import orient_oracle as oo
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(os.path.dirname(HERE))
-CSRC = os.path.join(ROOT, "imageflow_b200", "csrc")
+SOURCES = ("orient_kernel_emu.cc", "ifb_orient.cc")          # of tests.cpu_emu.build
 SIZES = [(1, 1), (1, 7), (7, 1), (5, 3), (31, 31), (32, 32), (33, 33), (31, 33), (33, 32), (1, 40), (40, 1), (65, 2), (2, 65)]
-
-
-def build(out_dir: str, sanitize: bool = False) -> str:
-    so = os.path.join(out_dir, "liborient_emu_asan.so" if sanitize else "liborient_emu.so")
-    cmd = ["g++", "-O1", "-g", "-std=c++17", "-shared", "-fPIC", "-Wall", "-Wno-unknown-pragmas"]
-    if sanitize:
-        cmd += ["-fsanitize=address", "-fno-omit-frame-pointer"]
-    subprocess.run(cmd + ["-o", so, os.path.join(HERE, "orient_kernel_emu.cc"), os.path.join(CSRC, "ifb_orient.cc")], check=True)
-    return so
 
 
 def load(so):

@@ -8,8 +8,6 @@ Every launch holds several jobs, each a sub-window of one larger bitmap filled w
   - the pixels stored are exactly the pixels the oracle writes (its touch mask);
   - the pixels loaded are pixels the oracle writes too (only blended pixels are read), each at most once."""
 import ctypes as C
-import os
-import subprocess
 import sys
 
 import numpy as np
@@ -18,18 +16,7 @@ import oracle
 from tests import round_corners_oracle as rco
 from imageflow_b200._lib import RoundCornersDesc
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(os.path.dirname(HERE))
-CSRC = os.path.join(ROOT, "imageflow_b200", "csrc")
-
-
-def build(out_dir: str, sanitize: bool = False) -> str:
-    so = os.path.join(out_dir, "librc_emu_asan.so" if sanitize else "librc_emu.so")
-    cmd = ["g++", "-O1", "-g", "-std=c++17", "-shared", "-fPIC", "-ffp-contract=off"]
-    if sanitize:
-        cmd += ["-fsanitize=address", "-fno-omit-frame-pointer"]
-    subprocess.run(cmd + ["-o", so, os.path.join(HERE, "round_corners_kernel_emu.cc"), os.path.join(CSRC, "ifb_round_corners.cc")], check=True)
-    return so
+SOURCES = ("round_corners_kernel_emu.cc", "ifb_round_corners.cc")          # of tests.cpu_emu.build
 
 
 def load(so):

@@ -13,8 +13,6 @@ oracle's (oracle.resample_stages), which the GPU's H pass equals bit for bit (te
   - no pixel is stored twice, and the pixels stored are exactly the rectangles of the jobs with pixels;
   - every load of a CTA is in its own job's rectangle or in its own group's F."""
 import ctypes as C
-import os
-import subprocess
 import sys
 
 import numpy as np
@@ -24,24 +22,12 @@ import oracle
 from imageflow_b200._lib import WatermarkDesc
 from tests import color_oracle as co
 from tests import watermark_oracle as wo
-from tests.cpu_emu import csr
+from tests.cpu_emu import csr, transfer_tables
 from tests.cpu_emu.run_orient_cases import Bitmap, window_in
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(os.path.dirname(HERE))
-CSRC = os.path.join(ROOT, "imageflow_b200", "csrc")
+SOURCES = ("watermark_kernel_emu.cc", "ifb_watermark.cc", "ifb_orient.cc")          # of tests.cpu_emu.build
 FILTERS = [2, 4, 13, 14, 6, 22]
 OPACITIES = [1.0, 1.0, float("nan"), 2.5, 0.7, 0.3, 0.0, -1.0]
-
-
-def build(out_dir: str, sanitize: bool = False) -> str:
-    so = os.path.join(out_dir, "libwatermark_emu_asan.so" if sanitize else "libwatermark_emu.so")
-    cmd = ["g++", "-O1", "-g", "-std=c++17", "-shared", "-fPIC", "-Wall", "-Wno-unknown-pragmas", "-ffp-contract=off"]
-    if sanitize:
-        cmd += ["-fsanitize=address", "-fno-omit-frame-pointer"]
-    subprocess.run(cmd + ["-o", so, os.path.join(HERE, "watermark_kernel_emu.cc"), os.path.join(CSRC, "ifb_watermark.cc"),
-                          os.path.join(CSRC, "ifb_orient.cc")], check=True)
-    return so
 
 
 def load(so):
@@ -61,11 +47,7 @@ _T = {}
 
 def tables():
     if not _T:
-        t_lin, t_srgb, lut = np.zeros(256, np.float32), np.zeros(256, np.float32), np.zeros(16384, np.uint8)
-        f32p, u8p = C.POINTER(C.c_float), C.POINTER(C.c_uint8)
-        ifb.lib().ifb200_byte_to_float_table(1, t_lin.ctypes.data_as(f32p)); ifb.lib().ifb200_byte_to_float_table(0, t_srgb.ctypes.data_as(f32p))
-        ifb.lib().ifb200_linear_to_srgb_table(lut.ctypes.data_as(u8p))
-        _T.update(lin=t_lin, srgb=t_srgb, lut=lut)
+        _T.update(zip(("lin", "srgb", "lut"), transfer_tables(ifb)))
     return _T
 
 

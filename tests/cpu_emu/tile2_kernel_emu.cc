@@ -1,73 +1,27 @@
 // Runs imageflow_b200/csrc/ifb_tile2_kernel.cuh -- the product's CUDA source of fused_tile2_kernel, unmodified -- on the CPU:
 // one OS thread per CUDA thread of a block, std::barrier for __syncthreads, a per-warp exchange for __reduce_max_sync, the CUDA
-// arithmetic intrinsics mapped onto IEEE host operations (built with -ffp-contract=off -frounding-math).  Blocks of the grid
+// arithmetic intrinsics mapped onto IEEE host operations (cuda_emu.h; built with -ffp-contract=off; the rounding mode stays
+// round-to-nearest, and __fadd_rz / __float2uint_rz round toward zero in software).  Blocks of the grid
 // run one after the other.  Dynamic shared memory is an exactly-sized heap block and every global buffer is whatever the
 // caller allocated, so building this file with -fsanitize=address turns a run into a memory check of the kernel.
 // TEST INFRASTRUCTURE: nothing in the product calls this; the GPU remains the place where the kernel is run and timed.
-#include <algorithm>
+#include "cuda_emu.h"
+
 #include <barrier>
-#include <cmath>
 #include <cstddef>
-#include <cstdint>
 #include <cstdlib>
-#include <cstring>
 #include <memory>
 #include <thread>
 #include <vector>
 
 namespace emu {
-struct Idx { unsigned x, y, z; };
-static thread_local Idx threadIdx;
-static Idx blockIdx, gridDim;
 static unsigned char* smem;
 static std::barrier<>* block_barrier;
 static std::barrier<>* warp_barrier[8];
 static unsigned warp_scratch[8][32];
 }  // namespace emu
-using emu::blockIdx;
-using emu::gridDim;
-#define threadIdx emu::threadIdx
-#define __global__
-#define __device__
-#define __host__
-#define __forceinline__ inline
-#define __restrict__
-#define __launch_bounds__(...)
 #define IFB_DYNAMIC_SMEM(name_) unsigned char* const name_ = emu::smem
 #define __syncthreads() emu::block_barrier->arrive_and_wait()
-using std::max;
-using std::min;
-struct alignas(16) float4 { float x, y, z, w; };
-struct alignas(16) uint4 { uint32_t x, y, z, w; };
-static inline float4 make_float4(float x, float y, float z, float w) { return float4{x, y, z, w}; }
-struct alignas(8) float2 { float x, y; };
-static inline float2 make_float2(float x, float y) { return float2{x, y}; }
-static inline uint32_t __float_as_uint(float f) { uint32_t u; std::memcpy(&u, &f, 4); return u; }
-static inline float __uint_as_float(uint32_t u) { float f; std::memcpy(&f, &u, 4); return f; }
-static inline float2 __fadd2_rn(float2 a, float2 b) { return float2{a.x + b.x, a.y + b.y}; }
-static inline uint32_t __byte_perm(uint32_t x, uint32_t y, uint32_t s) {
-    const uint64_t v = ((uint64_t)y << 32) | x; uint32_t r = 0;
-    for (int i = 0; i < 4; ++i) r |= (uint32_t)((v >> (8 * ((s >> (4 * i)) & 7))) & 0xff) << (8 * i);
-    return r;
-}
-template <class T> static inline T __ldg(const T* p) { return *p; }
-static inline float __fmaf_rn(float a, float b, float c) { return std::fmaf(a, b, c); }
-static inline float __fmul_rn(float a, float b) { return a * b; }
-static inline float __fadd_rn(float a, float b) { return a + b; }
-static inline float __fsub_rn(float a, float b) { return a - b; }
-static inline float __fdiv_rn(float a, float b) { return a / b; }
-static inline float __uint2float_rn(unsigned v) { return (float)v; }
-static inline float __fadd_rz(float a, float b) {          // add.rz.f32 without touching the thread's rounding mode (the compiler
-    const double s = (double)a + (double)b;                  // may move arithmetic across fesetround): the double sum is exact
-    float f = (float)s;                                      // for the operands met here; then round it toward zero
-    if (std::fabs((double)f) > std::fabs(s)) f = std::nextafterf(f, 0.0f);
-    return f;
-}
-static inline unsigned __float2uint_rz(float s) {           // cvt.rzi.u32.f32: NaN -> 0, saturating
-    if (!(s > 0.0f)) return 0u;
-    if (s >= 4294967296.0f) return 0xffffffffu;
-    return (unsigned)s;
-}
 static inline unsigned __reduce_max_sync(unsigned, unsigned v) {
     const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     emu::warp_scratch[warp][lane] = v;
@@ -85,7 +39,6 @@ namespace ifbk {
 #endif
 #include "../../imageflow_b200/csrc/ifb_tile2_kernel.cuh"
 }  // namespace ifbk
-#undef threadIdx
 
 using namespace ifbk;
 using KernelFn = void (*)(const JobDev*, uint32_t, Tables, AxisDev, AxisDev, TilePlanDev);
@@ -135,6 +88,7 @@ extern "C" int emu_tile2_launch(int ch, int linear, int compose, int cm, unsigne
                 fn(static_cast<const JobDev*>(jobs), n_jobs, tb, av, ah, pl);
             });
         for (auto& x : th) x.join();
+        emu::block_barrier = nullptr;
     }
     return 0;
 }

@@ -5,12 +5,10 @@
 // run one after the other.  Every canvas and F access of the composite goes through IFB_WM_LOAD* / IFB_WM_STORE*, which record the
 // address of each 4-byte word they touch (a 16-byte pixel access records its four pixels; an F load records the pixel's first word)
 // together with the CTA that made it.
-#include <algorithm>
-#include <cmath>
+#include "cuda_emu.h"
+
 #include <cstddef>
-#include <cstdint>
 #include <cstdio>
-#include <cstring>
 #include <string>
 #include <vector>
 
@@ -18,8 +16,6 @@
 #include "../../imageflow_b200/csrc/ifb_watermark.h"
 
 namespace emu {
-struct Idx { unsigned x, y, z; };
-static Idx threadIdx, blockIdx, blockDim, gridDim;
 static std::vector<uint64_t> loads, stores;            // (address, CTA) pairs, flattened
 template <class T> static void rec(std::vector<uint64_t>& v, const T* p, size_t words) {
     for (size_t i = 0; i < words; ++i) { v.push_back((uint64_t)(uintptr_t)p + 4 * i); v.push_back(blockIdx.x); }
@@ -28,27 +24,6 @@ template <class T> static T load(const T* p) { rec(loads, p, sizeof(T) / 4); ret
 template <class T> static T loadf(const T* p) { rec(loads, p, 1); return *p; }
 template <class T> static void store(T* p, const T& v) { rec(stores, p, sizeof(T) / 4); *p = v; }
 }  // namespace emu
-#define __global__
-#define __device__
-#define __forceinline__ inline
-#define __restrict__
-#define __launch_bounds__(...)
-using emu::blockDim;
-using emu::blockIdx;
-using emu::gridDim;
-using emu::threadIdx;
-struct uint4 { uint32_t x, y, z, w; };
-struct float4 { float x, y, z, w; };
-static inline uint4 make_uint4(uint32_t x, uint32_t y, uint32_t z, uint32_t w) { return {x, y, z, w}; }
-static inline float4 make_float4(float x, float y, float z, float w) { return {x, y, z, w}; }
-template <class T> static inline T __ldg(const T* p) { return *p; }
-static inline float __fmaf_rn(float a, float b, float c) { return std::fmaf(a, b, c); }
-static inline float __fmul_rn(float a, float b) { return a * b; }
-static inline float __fadd_rn(float a, float b) { return a + b; }
-static inline float __fsub_rn(float a, float b) { return a - b; }
-static inline float __fdiv_rn(float a, float b) { return a / b; }
-using std::max;
-using std::min;
 #define IFB_WM_LOAD4(p) emu::load(p)
 #define IFB_WM_STORE4(p, v) emu::store(p, (uint32_t)(v))
 #define IFB_WM_LOAD16(p) emu::load(p)
@@ -62,34 +37,21 @@ namespace ifbk {
 #include "../../imageflow_b200/csrc/ifb_watermark_kernel.cuh"
 }  // namespace ifbk
 
-namespace {
-bool check_and_plan(const ifb200_watermark_desc* d, size_t n, const float* t_lin, const float* t_srgb, ifb::WmWork& wk, char* err,
-                    size_t err_cap, long* code) {
-    for (size_t i = 0; i < n; ++i) {
-        int c = 0;
-        const std::string why = ifb::watermark_check(d[i], &c);
-        if (!why.empty()) {
-            snprintf(err, err_cap, "watermark job %zu: %s", i, why.c_str());
-            *code = -c;
-            return false;
-        }
-    }
-    ifb::watermark_plan(d, n, t_lin, t_srgb, wk);
-    return true;
-}
-}  // namespace
-
-// The plan of a call, as ifb200_batch_watermark makes it: every descriptor checked, then grouped.  groups: 8 words per group (w, h,
-// rows, tiles, job0, n, first, F byte offset); rep: the descriptor index of each group; opacity: what each group's copy gets (>= 1: none);
-// jobs: 4 words per job (out address low, high, stride, groups).  Returns the CTAs of the composite, or -(ifb200_status) when a descriptor
+// The plan of a call, as ifb200_batch_watermark makes it: watermark_prepare, which watermark_locked (ifb_engine.cu) calls too.
+// groups: 8 words per group (w, h, rows, tiles, job0, n, first, F byte offset); rep: the descriptor index of each group; opacity: what
+// each group's copy gets (>= 1: none); jobs: 4 words per job (out address low, high, stride, groups).  Returns the CTAs of the composite, or -(ifb200_status) when a descriptor
 // is rejected (err = why).
 extern "C" long emu_watermark_plan(const ifb200_watermark_desc* d, size_t n, const float* t_lin, const float* t_srgb, uint32_t* groups,
                                    uint32_t* rep, float* opacity, size_t g_cap, uint32_t* jobs, size_t j_cap, size_t* n_groups,
                                    size_t* n_jobs, char* err, size_t err_cap) {
     ifb::WmWork wk;
-    long code = 0;
+    int code = 0;
     *n_groups = *n_jobs = 0;
-    if (!check_and_plan(d, n, t_lin, t_srgb, wk, err, err_cap, &code)) return code;
+    const std::string why = ifb::watermark_prepare(d, n, t_lin, t_srgb, wk, &code);
+    if (!why.empty()) {
+        snprintf(err, err_cap, "%s", why.c_str());
+        return -code;
+    }
     *n_groups = wk.groups.size(); *n_jobs = wk.jobs.size();
     for (size_t g = 0; g < wk.groups.size() && g < g_cap; ++g) {
         const ifb::WmGroup& q = wk.groups[g];
@@ -116,9 +78,13 @@ extern "C" long emu_watermark(const ifb200_watermark_desc* d, size_t n, const fl
                               uint64_t* loads, uint64_t* stores, size_t cap, size_t* n_loads, size_t* n_stores, char* err, size_t err_cap,
                               int sabotage) {
     ifb::WmWork wk;
-    long code = 0;
+    int code = 0;
     *n_loads = *n_stores = 0;
-    if (!check_and_plan(d, n, t_lin, t_srgb, wk, err, err_cap, &code)) return code;
+    const std::string why = ifb::watermark_prepare(d, n, t_lin, t_srgb, wk, &code);
+    if (!why.empty()) {
+        snprintf(err, err_cap, "%s", why.c_str());
+        return -code;
+    }
     for (auto& g : wk.groups) g.f = reinterpret_cast<const float*>(reinterpret_cast<uint8_t*>(F) + (uintptr_t)g.f);
     const ifbk::Tables tb{t_lin, t_srgb, lut16k};
     for (size_t g = 0; g < wk.groups.size(); ++g) {

@@ -4,28 +4,13 @@
 //   threads of a block run one after the other; the kernel has ONE __syncthreads(), which is emulated by running every
 //   thread twice: pass 0 returns at the barrier (the shared tile gets filled), pass 1 runs through (each thread rewrites
 //   the same tile values, then computes its pixel).
-#include <algorithm>
-#include <cstdint>
-#include <cstdlib>
-#include <cstddef>
+#include "cuda_emu.h"
 
 namespace emu {
-struct Idx { unsigned x, y, z; };
-static Idx threadIdx, blockIdx;
 static int pass;
 }  // namespace emu
-#define __global__
-#define __device__
-#define __forceinline__ inline
-#define __restrict__
-#define __launch_bounds__(...)
 #define __shared__ static
 #define __syncthreads() do { if (emu::pass == 0) return; } while (0)
-using emu::blockIdx;
-using emu::threadIdx;
-using std::max;
-using std::min;
-template <class T> static inline T __ldg(const T* p) { return *p; }
 
 namespace ifbk {
 #include "../../imageflow_b200/csrc/ifb_whitespace_kernel.cuh"

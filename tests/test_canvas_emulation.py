@@ -4,20 +4,15 @@ as the engine does: multi-job calls mixing all four ops in exactly sized bitmaps
 for results, for the set of pixels written (each once) and for the pixels read (tests/cpu_emu/run_canvas_cases.py); then the same
 under AddressSanitizer; and plans corrupted on purpose, which the checks must reject.  The kernel is also run on the GPU
 (tests/test_canvas_gpu.py)."""
-import os
-import subprocess
-import sys
-
 import pytest
 
+from tests import cpu_emu
 from tests.cpu_emu import run_canvas_cases
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
 def emu_so(tmp_path_factory):
-    return run_canvas_cases.build(str(tmp_path_factory.mktemp("canvas_emu")))
+    return cpu_emu.build(str(tmp_path_factory.mktemp("canvas_emu")), *run_canvas_cases.SOURCES)
 
 
 def test_emulated_canvas_kernel_matches_the_oracle(emu_so):
@@ -30,11 +25,6 @@ def test_a_sabotaged_plan_is_caught(emu_so, kind):
 
 
 def test_emulated_canvas_kernel_under_address_sanitizer(tmp_path):
-    asan = subprocess.run(["g++", "-print-file-name=libasan.so"], capture_output=True, text=True).stdout.strip()
-    if not os.path.isabs(asan) or not os.path.exists(asan):
-        pytest.skip("libasan not available")
-    so = run_canvas_cases.build(str(tmp_path), sanitize=True)
-    env = dict(os.environ, LD_PRELOAD=asan, ASAN_OPTIONS="detect_leaks=0:verify_asan_link_order=0", PYTHONPATH=ROOT)
-    r = subprocess.run([sys.executable, "-m", "tests.cpu_emu.run_canvas_cases", so, "150"], capture_output=True, text=True, cwd=ROOT,
-                       env=env, timeout=1200)
+    so = cpu_emu.build(str(tmp_path), *run_canvas_cases.SOURCES, sanitize=True)
+    r = cpu_emu.run_under_asan("run_canvas_cases", so, 150)
     assert r.returncode == 0 and "cases bit-exact:" in r.stdout and "AddressSanitizer" not in r.stderr, (r.stdout[-300:], r.stderr[-1500:])

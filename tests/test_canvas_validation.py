@@ -8,6 +8,7 @@ import pytest
 
 import imageflow_b200 as ifb
 from imageflow_b200._lib import CanvasDesc
+from tests import cpu_emu
 from tests.cpu_emu import run_canvas_cases as rcc
 
 FILL, COPY, EXPAND, NORMALIZE = range(4)
@@ -15,7 +16,7 @@ FILL, COPY, EXPAND, NORMALIZE = range(4)
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return rcc.load(rcc.build(str(tmp_path_factory.mktemp("canvas_emu"))))
+    return rcc.load(cpu_emu.build(str(tmp_path_factory.mktemp("canvas_emu")), *rcc.SOURCES))
 
 
 def _call(L, descs):

@@ -4,20 +4,15 @@ exactly as the engine does: multi-job calls of random chains, with and without w
 of sentinel bytes at every 4-byte phase modulo 16, checked for results, for the pixels stored (each once), for the pixels loaded and
 for the white balance's histograms (tests/cpu_emu/run_color_cases.py); then the same under AddressSanitizer; and plans corrupted on
 purpose, which the checks must reject.  The kernels are also run on the GPU (tests/test_color_chain_gpu.py)."""
-import os
-import subprocess
-import sys
-
 import pytest
 
+from tests import cpu_emu
 from tests.cpu_emu import run_color_cases
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
 def emu_so(tmp_path_factory):
-    return run_color_cases.build(str(tmp_path_factory.mktemp("color_emu")))
+    return cpu_emu.build(str(tmp_path_factory.mktemp("color_emu")), *run_color_cases.SOURCES)
 
 
 def test_emulated_color_kernels_match_the_node_by_node_chain(emu_so):
@@ -30,11 +25,6 @@ def test_a_sabotaged_plan_is_caught(emu_so, kind):
 
 
 def test_emulated_color_kernels_under_address_sanitizer(tmp_path):
-    asan = subprocess.run(["g++", "-print-file-name=libasan.so"], capture_output=True, text=True).stdout.strip()
-    if not os.path.isabs(asan) or not os.path.exists(asan):
-        pytest.skip("libasan not available")
-    so = run_color_cases.build(str(tmp_path), sanitize=True)
-    env = dict(os.environ, LD_PRELOAD=asan, ASAN_OPTIONS="detect_leaks=0:verify_asan_link_order=0", PYTHONPATH=ROOT)
-    r = subprocess.run([sys.executable, "-m", "tests.cpu_emu.run_color_cases", so, "80"], capture_output=True, text=True, cwd=ROOT,
-                       env=env, timeout=1200)
+    so = cpu_emu.build(str(tmp_path), *run_color_cases.SOURCES, sanitize=True)
+    r = cpu_emu.run_under_asan("run_color_cases", so, 80)
     assert r.returncode == 0 and "cases bit-exact:" in r.stdout and "AddressSanitizer" not in r.stderr, (r.stdout[-300:], r.stderr[-1500:])

@@ -11,6 +11,7 @@ import pytest
 import imageflow_b200 as ifb
 from imageflow_b200._lib import ColorDesc
 from tests import color_oracle as co
+from tests import cpu_emu
 from tests.cpu_emu import run_color_cases as rcc
 
 TABLE, MATRIX, WB = 0, 1, 2
@@ -18,7 +19,7 @@ TABLE, MATRIX, WB = 0, 1, 2
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return rcc.load(rcc.build(str(tmp_path_factory.mktemp("color_emu"))))
+    return rcc.load(cpu_emu.build(str(tmp_path_factory.mktemp("color_emu")), *rcc.SOURCES))
 
 
 def _call(L, descs):

@@ -9,12 +9,13 @@ import pytest
 
 import imageflow_b200 as ifb
 from imageflow_b200._lib import OrientDesc
+from tests import cpu_emu
 from tests.cpu_emu import run_orient_cases as roc
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return roc.load(roc.build(str(tmp_path_factory.mktemp("orient_emu"))))
+    return roc.load(cpu_emu.build(str(tmp_path_factory.mktemp("orient_emu")), *roc.SOURCES))
 
 
 def _call(L, descs):

@@ -5,20 +5,15 @@ opacity case, compose mode, format and working space, on sub-windows of exactly 
 checked for F, for the results, for the pixels stored (each once), for the loads (only the job's rectangle and its group's F) and for
 the bytes around the rectangles (tests/cpu_emu/run_watermark_cases.py); then the same under AddressSanitizer; and plans corrupted on
 purpose, which the checks must reject.  The kernels also run on the GPU (tests/test_watermark_gpu.py)."""
-import os
-import subprocess
-import sys
-
 import pytest
 
+from tests import cpu_emu
 from tests.cpu_emu import run_watermark_cases
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
 def emu_so(tmp_path_factory):
-    return run_watermark_cases.build(str(tmp_path_factory.mktemp("watermark_emu")))
+    return cpu_emu.build(str(tmp_path_factory.mktemp("watermark_emu")), *run_watermark_cases.SOURCES)
 
 
 def test_emulated_watermark_kernels_match_the_node_by_node_expansion(emu_so):
@@ -35,11 +30,6 @@ def test_an_unsabotaged_sabotage_case_passes(emu_so):
 
 
 def test_emulated_watermark_kernels_under_address_sanitizer(tmp_path):
-    asan = subprocess.run(["g++", "-print-file-name=libasan.so"], capture_output=True, text=True).stdout.strip()
-    if not os.path.isabs(asan) or not os.path.exists(asan):
-        pytest.skip("libasan not available")
-    so = run_watermark_cases.build(str(tmp_path), sanitize=True)
-    env = dict(os.environ, LD_PRELOAD=asan, ASAN_OPTIONS="detect_leaks=0:verify_asan_link_order=0", PYTHONPATH=ROOT)
-    r = subprocess.run([sys.executable, "-m", "tests.cpu_emu.run_watermark_cases", so, "25"], capture_output=True, text=True, cwd=ROOT,
-                       env=env, timeout=1200)
+    so = cpu_emu.build(str(tmp_path), *run_watermark_cases.SOURCES, sanitize=True)
+    r = cpu_emu.run_under_asan("run_watermark_cases", so, 25)
     assert r.returncode == 0 and "cases bit-exact:" in r.stdout and "AddressSanitizer" not in r.stderr, (r.stdout[-300:], r.stderr[-1500:])

@@ -59,12 +59,8 @@ def test_kernel_source_under_cpu_emulation_matches_the_oracle(tmp_path):
     g++ under a sequential emulation of threadIdx / blockIdx / __shared__ / __syncthreads and runs it with the launch geometry
     the engine uses: every code byte must equal the oracle's, for ragged sizes, padded pitches, both grayscale formulas."""
     import ctypes as C
-    import os
-    import subprocess
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    so = str(tmp_path / "libws_emu.so")
-    subprocess.run(["g++", "-O2", "-shared", "-fPIC", "-std=c++17", "-o", so, os.path.join(root, "tests", "cpu_emu", "whitespace_kernel_emu.cc")], check=True)
-    L = C.CDLL(so)
+    from tests import cpu_emu
+    L = C.CDLL(cpu_emu.build(str(tmp_path), "whitespace_kernel_emu.cc"))
     L.emu_whitespace_codes.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_void_p]
     for a, thr, am in _images(200, 5):
         h, w = a.shape[:2]
