@@ -18,6 +18,8 @@ Host-side mirror of the reference seam (paths relative to the imageflow checkout
       WhiteBalanceHistogramAreaThresholdSrgb as one chain per frame (Batch.color_chain; RIAPI's s.* / a.balancewhite as riapi_color_steps)
   flow/nodes/watermark.rs, imageflow_riapi ir4/layout.rs + sizing.rs  Watermark: its layout (watermark_layout, process_constraint) and
       every frame's composite from one resample per distinct watermark (Batch.watermark; RIAPI's placement as riapi_watermark_placement)
+  graphics/swizzle.rs, bitmaps.rs:1284-1345  rgb_to_bgra, copy_swap_br, gray_to_bgra, gray_alpha_to_bgra, to_vec_rgb: decoder rows into
+      BGRA and encoder rows out of it, batched (Batch.pixel_convert over PixelRows; Batch.to_bgra / from_bgra for one tensor)
   c_components/lib/codecs_jpeg_idct_fast.c  flow_scale_spatial[_srgb]_NxN (decode-time JPEG block scalers)
 All arithmetic runs in hand-written sm_90a kernels inside libifb200.so (include/ifb200.h);
 this package only marshals arguments.  Nothing here imports the CPU oracle.
@@ -31,7 +33,8 @@ from .graphics import (Batch, apply_matte, BitmapCompositing, BitmapWindow, Erro
                        ApplyOrientation, Rotate90, Rotate180, Rotate270, FlipH, FlipV, Transpose, orientation_of, riapi_rotate_steps,
                        riapi_flip_steps, apply_orientation, ColorMatrixSrgb, ColorFilterSrgb, WhiteBalanceHistogramAreaThresholdSrgb,
                        riapi_color_steps, Watermark, WatermarkConstraintBox, WatermarkConstraintMode, ConstraintGravity, WatermarkDraw,
-                       process_constraint, watermark_layout, riapi_watermark_placement)
+                       process_constraint, watermark_layout, riapi_watermark_placement, PixelRows, RgbToBgra, RgbaToBgra, GrayToBgra,
+                       GrayAlphaToBgra, BgraToRgb, pixel_op_for)
 from ._lib import LIB_PATH, ResampleDesc, lib
 
 __all__ = [
@@ -44,5 +47,6 @@ __all__ = [
     "ApplyOrientation", "Rotate90", "Rotate180", "Rotate270", "FlipH", "FlipV", "Transpose", "orientation_of", "riapi_rotate_steps",
     "riapi_flip_steps", "apply_orientation", "ColorMatrixSrgb", "ColorFilterSrgb", "WhiteBalanceHistogramAreaThresholdSrgb",
     "riapi_color_steps", "Watermark", "WatermarkConstraintBox", "WatermarkConstraintMode", "ConstraintGravity", "WatermarkDraw",
-    "process_constraint", "watermark_layout", "riapi_watermark_placement", "LIB_PATH", "ResampleDesc", "lib",
+    "process_constraint", "watermark_layout", "riapi_watermark_placement", "PixelRows", "RgbToBgra", "RgbaToBgra", "GrayToBgra",
+    "GrayAlphaToBgra", "BgraToRgb", "pixel_op_for", "LIB_PATH", "ResampleDesc", "lib",
 ]

@@ -22,6 +22,7 @@ SYMBOLS = [
     "ifb200_batch_fused_jobs", "ifb200_batch_generic_jobs", "ifb200_batch_tile_jobs", "ifb200_batch_ring_status", "ifb200_hv_plan_tables",
     "ifb200_block_scale_u8", "ifb200_batch_block_scale", "ifb200_round_corners_bgra8", "ifb200_batch_round_corners",
     "ifb200_batch_canvas", "ifb200_batch_orient", "ifb200_batch_color_chain", "ifb200_batch_watermark",
+    "ifb200_batch_pixel_convert",
 ]
 
 
@@ -80,6 +81,14 @@ class ColorDesc(C.Structure):
 class WatermarkDesc(C.Structure):
     """struct ifb200_watermark_desc"""
     _fields_ = [("draw", ResampleDesc), ("opacity", C.c_float)]
+
+
+class PixelConvertDesc(C.Structure):
+    """struct ifb200_pixel_convert_desc"""
+    _fields_ = [
+        ("op", C.c_int32), ("src", C.c_void_p), ("src_stride", C.c_uint32), ("dst", C.c_void_p), ("dst_stride", C.c_uint32),
+        ("w", C.c_uint32), ("h", C.c_uint32), ("opaque", C.c_int32),
+    ]
 
 
 _lib = None
@@ -176,6 +185,8 @@ def lib() -> C.CDLL:
     L.ifb200_batch_color_chain.restype = C.c_int
     L.ifb200_batch_watermark.argtypes = [C.c_void_p, C.POINTER(WatermarkDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_watermark.restype = C.c_int
+    L.ifb200_batch_pixel_convert.argtypes = [C.c_void_p, C.POINTER(PixelConvertDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
+    L.ifb200_batch_pixel_convert.restype = C.c_int
     L.ifb200_batch_ring_status.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_ring_status.restype = C.c_int
     _lib = L

@@ -1246,6 +1246,24 @@ void orient_locked(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, cudaS
     b->launches++;
 }
 
+// The conversions of ifb200_batch_pixel_convert (ifb_pixel_convert.h): every descriptor is checked before anything is planned or
+// enqueued, then all jobs run in ONE launch (none when no job has pixels).  The upload is the items and their first CTAs, O(jobs).
+void pixel_convert_locked(ifb200_batch* b, const ifb200_pixel_convert_desc* d, size_t n, cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    ifb::PcWork wk;
+    int code = 0;
+    const std::string why = ifb::pixel_convert_prepare(d, n, wk, &code);
+    if (!why.empty()) IFB_THROW(code, "%s", why.c_str());
+    if (wk.items.empty()) return;
+    if (wk.ctas() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
+    DeviceScope dev_scope_(b->device);
+    WorkUpload up(b, st, {part(wk.items), part(wk.first)});
+    pixel_convert_kernel<<<(unsigned)wk.ctas(), ifb::kPcThreads, 0, st>>>(up.at<const ifb::PcItem>(0), up.at<const uint32_t>(1),
+                                                                           (uint32_t)wk.items.size());
+    CUDA_OK(cudaGetLastError());
+    b->launches++;
+}
+
 // The colour chains of ifb200_batch_color_chain (ifb_color.h): every descriptor is checked before anything is planned or enqueued.
 // The plan (jobs, prefix sums, segments, tables, matrices) goes up in one copy, O(jobs + steps); then ONE launch, or three when some
 // job white-balances (histograms into zeroed counters, byte maps into the jobs' kClWb tables, apply); none when no job writes a pixel.
@@ -1783,6 +1801,10 @@ int ifb200_batch_canvas(ifb200_batch* b, const ifb200_canvas_desc* d, size_t n, 
 
 int ifb200_batch_orient(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, void* stream, char* err, size_t cap) {
     return with_batch(b, stream, err, cap, [&](cudaStream_t st) { orient_locked(b, d, n, st); });
+}
+
+int ifb200_batch_pixel_convert(ifb200_batch* b, const ifb200_pixel_convert_desc* d, size_t n, void* stream, char* err, size_t cap) {
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { pixel_convert_locked(b, d, n, st); });
 }
 
 int ifb200_batch_color_chain(ifb200_batch* b, const ifb200_color_desc* d, size_t n, void* stream, char* err, size_t cap) {

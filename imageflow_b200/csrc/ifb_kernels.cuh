@@ -23,6 +23,7 @@
 #include "ifb_orient.h"            // OrItem: planned on the host, read by orient_kernel
 #include "ifb_color.h"             // ClJob / ClSeg: planned on the host, read by the colour-chain kernels
 #include "ifb_watermark.h"         // WmJob / WmGroup: planned on the host, read by watermark_composite_kernel
+#include "ifb_pixel_convert.h"     // PcItem: planned on the host, read by pixel_convert_kernel
 
 namespace ifbk {
 
@@ -298,6 +299,9 @@ __global__ void __launch_bounds__(256) apply_byte_maps_bgra8_kernel(uint8_t* __r
 
 // ---------------------------------------------------------------- orientation (ApplyOrientation, rotations, flips, transpose) as one gather; own file for tests/cpu_emu
 #include "ifb_orient_kernel.cuh"
+
+// ---------------------------------------------------------------- pixel formats at the graph's edges (RGB24, RGBA, Gray, GrayAlpha <-> BGRA); own file for tests/cpu_emu
+#include "ifb_pixel_convert_kernel.cuh"
 
 // ---------------------------------------------------------------- decode-time JPEG block scalers (SURVEY.md section 8(f), item 1)
 #include "ifb_idct_kernel.cuh"

@@ -9,7 +9,7 @@ from typing import Optional, Sequence
 
 import numpy as np
 
-from ._lib import CanvasDesc, ColorDesc, ColorStep, OrientDesc, ResampleDesc, RoundCornersDesc, WatermarkDesc, lib
+from ._lib import CanvasDesc, ColorDesc, ColorStep, OrientDesc, PixelConvertDesc, ResampleDesc, RoundCornersDesc, WatermarkDesc, lib
 
 
 class Filter(enum.IntEnum):
@@ -963,6 +963,114 @@ def plan_probe(geometries, threads: int = 1, want_hash: bool = False) -> dict:
     return {"seconds": sec.value, "table_bytes": nb.value, "table_hash": hs.value if want_hash else None}
 
 
+# ---------------------------------------------------------------- pixel formats at the graph's edges (Batch.pixel_convert)
+@dataclass
+class PixelRows:
+    """Rows of 1, 2, 3 or 4 interleaved uint8 channels (Gray8, GrayAlpha8, RGB24, RGBA32 or BGRA32) at any row stride and any byte
+    offset: what a decoder hands over and an encoder takes.  Host (numpy) or device (raw pointer) memory, like BitmapWindow."""
+    ptr: int
+    w: int
+    h: int
+    stride: int
+    channels: int
+    _keep: object = field(default=None, repr=False)
+
+    @staticmethod
+    def _of(ptr, shape, strides, keep) -> "PixelRows":
+        if len(shape) != 3 or shape[2] not in (1, 2, 3, 4) or strides[2] != 1 or strides[1] != shape[2] or strides[0] < 0:
+            raise FlowError(ErrorKind.InvalidArgument, f"pixel rows must be (H, W, C) uint8 with C in 1..4, interleaved, rows of any "
+                                                       f"non-negative stride; got shape {tuple(shape)}, strides {tuple(strides)}")
+        return PixelRows(ptr, shape[1], shape[0], strides[0], shape[2], keep)
+
+    @staticmethod
+    def from_numpy(a: np.ndarray) -> "PixelRows":
+        if a.dtype != np.uint8:
+            raise FlowError(ErrorKind.InvalidArgument, f"pixel rows must be uint8, not {a.dtype}")
+        return PixelRows._of(a.ctypes.data, a.shape, a.strides, a)
+
+    @staticmethod
+    def from_torch(t) -> "PixelRows":
+        """t: uint8 CUDA tensor of shape (H, W, C), e.g. nvJPEG's interleaved RGB; a CHW tensor needs .permute(1, 2, 0).contiguous()."""
+        import torch
+        if t.dtype != torch.uint8:
+            raise FlowError(ErrorKind.InvalidArgument, f"pixel rows must be uint8, not {t.dtype}")
+        return PixelRows._of(t.data_ptr(), tuple(t.shape), t.stride(), t)
+
+    @staticmethod
+    def of(x) -> "PixelRows":
+        """PixelRows of a numpy array, a torch tensor, a BitmapWindow (4 channels) or PixelRows"""
+        if isinstance(x, PixelRows):
+            return x
+        if isinstance(x, BitmapWindow):
+            return PixelRows(x.ptr, x.w, x.h, x.stride, 4, x._keep)
+        return PixelRows.from_numpy(x) if isinstance(x, np.ndarray) else PixelRows.from_torch(x)
+
+
+# op -> (source channels, destination channels), include/ifb200.h enum ifb200_pixel_op
+_PIXEL_OP_CHANNELS = {0: (3, 4), 1: (4, 4), 2: (1, 4), 3: (2, 4), 4: (4, 3)}
+
+
+@dataclass
+class RgbToBgra:
+    """rgb_to_bgra (graphics/swizzle.rs:26-31): RGB24 rows -> BGRA, alpha 255 (image_png_decoder.rs, jpeg_decoder.rs)."""
+    src: object
+    dst: object
+    opaque: bool = False
+    OP = 0
+
+
+@dataclass
+class RgbaToBgra:
+    """copy_swap_br (graphics/swizzle.rs:14-19): bytes 0 and 2 swapped, so RGBA -> BGRA and BGRA -> RGBA alike.  dst None = in place
+    (swap_br_inplace, :8-12); opaque = alpha 255 (the encoders' swap then fill, zen_encoder.rs:585-603, in one pass)."""
+    src: object
+    dst: object = None
+    opaque: bool = False
+    OP = 1
+
+
+@dataclass
+class GrayToBgra:
+    """gray_to_bgra (graphics/swizzle.rs:33-37): Gray8 rows -> (v, v, v, 255)."""
+    src: object
+    dst: object
+    opaque: bool = False
+    OP = 2
+
+
+@dataclass
+class GrayAlphaToBgra:
+    """gray_alpha_to_bgra (graphics/swizzle.rs:39-45): GrayAlpha8 rows -> (v, v, v, a); opaque = alpha 255."""
+    src: object
+    dst: object
+    opaque: bool = False
+    OP = 3
+
+
+@dataclass
+class BgraToRgb:
+    """to_vec_rgb (graphics/bitmaps.rs:1316-1345): BGRA -> RGB24 rows, alpha dropped without a matte."""
+    src: object
+    dst: object
+    opaque: bool = False
+    OP = 4
+
+
+_PIXEL_OPS = {c.OP: c for c in (RgbToBgra, RgbaToBgra, GrayToBgra, GrayAlphaToBgra, BgraToRgb)}
+_PIXEL_DESC_DTYPE = np.dtype({"names": [n for n, _ in PixelConvertDesc._fields_],
+                              "formats": [np.uint64 if t is C.c_void_p else np.dtype(t) for n, t in PixelConvertDesc._fields_],
+                              "offsets": [getattr(PixelConvertDesc, n).offset for n, _ in PixelConvertDesc._fields_],
+                              "itemsize": C.sizeof(PixelConvertDesc)})
+
+
+def pixel_op_for(channels: int, to_bgra: bool = True):
+    """The record that converts rows of `channels` channels into BGRA (to_bgra) or BGRA into them (3: BgraToRgb, 4: RgbaToBgra)."""
+    ops = {1: GrayToBgra, 2: GrayAlphaToBgra, 3: RgbToBgra, 4: RgbaToBgra} if to_bgra else {3: BgraToRgb, 4: RgbaToBgra}
+    if channels not in ops:
+        raise FlowError(ErrorKind.InvalidArgument, f"no conversion {'from' if to_bgra else 'to'} {channels}-channel rows")
+    return ops[channels]
+
+
 def device_count() -> int:
     return lib().ifb200_device_count()
 
@@ -1120,6 +1228,62 @@ class Batch:
             out.alpha_meaningful = inp.alpha_meaningful
         self._keep.append([(j[0]._keep, o._keep) for j, o in zip(jobs, outs)])
         return outs
+
+    def pixel_convert(self, jobs, stream=None) -> list:
+        """Pixel-format conversions on DEVICE rows, all jobs in one kernel launch (none when no job has pixels), asynchronous on
+        `stream`.  jobs: iterable of RgbToBgra, RgbaToBgra, GrayToBgra, GrayAlphaToBgra and BgraToRgb records, whose src and dst are
+        BitmapWindows (BGRA) or anything PixelRows.of() takes, with the channels the op reads and writes.  No job may write what
+        another job of the call reads or writes.  Returns the destinations (the source for an in-place RgbaToBgra); a BitmapWindow
+        destination gets alpha_meaningful as a decoder sets it (RGBA and GrayAlpha sources, unless opaque).  Nothing is changed when
+        an argument is rejected."""
+        jobs = list(jobs)
+        srcs, dsts = [], []
+        for j in jobs:
+            if not isinstance(j, tuple(_PIXEL_OPS.values())):
+                raise FlowError(ErrorKind.InvalidArgument, f"not a pixel conversion: {j!r}")
+            dst = j.src if j.dst is None else j.dst
+            s, d = PixelRows.of(j.src), PixelRows.of(dst)
+            cs, cd = _PIXEL_OP_CHANNELS[j.OP]
+            if (s.channels, d.channels) != (cs, cd) or (s.w, s.h) != (d.w, d.h):
+                raise FlowError(ErrorKind.InvalidArgument, f"{type(j).__name__} converts {cs}-channel rows into {cd}-channel rows of the "
+                                                           f"same size, not {s.w}x{s.h}x{s.channels} into {d.w}x{d.h}x{d.channels}")
+            srcs.append(s); dsts.append(d)
+        a = np.zeros(len(jobs), _PIXEL_DESC_DTYPE)                # filled a column at a time: no per-field ctypes marshalling
+        a["op"] = [j.OP for j in jobs]; a["opaque"] = [int(bool(j.opaque)) for j in jobs]
+        a["src"] = [s.ptr for s in srcs]; a["src_stride"] = [s.stride for s in srcs]
+        a["dst"] = [d.ptr for d in dsts]; a["dst_stride"] = [d.stride for d in dsts]
+        a["w"] = [s.w for s in srcs]; a["h"] = [s.h for s in srcs]
+        arr = (PixelConvertDesc * len(jobs)).from_buffer(a)
+        buf = C.create_string_buffer(512)
+        _check(lib().ifb200_batch_pixel_convert(self._h, arr, len(jobs), self._stream(stream), buf, 512), buf)
+        out = []
+        for j in jobs:
+            dst = j.src if j.dst is None else j.dst
+            if isinstance(dst, BitmapWindow) and j.OP != BgraToRgb.OP:
+                dst.alpha_meaningful = j.OP in (RgbaToBgra.OP, GrayAlphaToBgra.OP) and not j.opaque
+            out.append(dst)
+        self._keep.append([(s._keep, d._keep) for s, d in zip(srcs, dsts)])
+        return out
+
+    def to_bgra(self, rows, opaque: bool = False, stream=None) -> "BitmapWindow":
+        """One call from decoder rows -- an (H, W, C) uint8 CUDA tensor, C in 1..4, or PixelRows -- to a new BGRA BitmapWindow on the
+        batch's device (a torch tensor with rows padded to 64 bytes, as bitmaps.rs:803-804)."""
+        import torch
+        s = PixelRows.of(rows)
+        op = pixel_op_for(s.channels)
+        pitch = (s.w * 4 + 63) // 64 * 64
+        t = torch.empty((s.h, pitch // 4, 4), dtype=torch.uint8, device=f"cuda:{self.device}")[:, :s.w]
+        win = BitmapWindow.from_torch(t)
+        self.pixel_convert([op(s, win, opaque)], stream)
+        return win
+
+    def from_bgra(self, window: "BitmapWindow", channels: int = 3, opaque: bool = False, stream=None):
+        """One call from a BGRA window to a new contiguous (H, W, channels) uint8 CUDA tensor: RGB24 (3) or RGBA32 (4) rows, as an
+        encoder takes them."""
+        import torch
+        t = torch.empty((window.h, window.w, channels), dtype=torch.uint8, device=f"cuda:{self.device}")
+        self.pixel_convert([pixel_op_for(channels, to_bgra=False)(window, t, opaque)], stream)
+        return t
 
     def color_chain(self, jobs, stream=None) -> list:
         """Colour chains on DEVICE windows, in place, all jobs in one kernel launch (three when a job white-balances; none when no

@@ -257,6 +257,29 @@ typedef struct ifb200_watermark_desc {
     float opacity;
 } ifb200_watermark_desc;
 
+/* One pixel-format conversion at the edge of a flow graph: the row swizzles of graphics/swizzle.rs:8-45 that the decoders call into
+ * BGRA (image_png_decoder.rs:156-193, jpeg_decoder.rs:103-129) and the RGB rows the encoders take out of it (bitmaps.rs:1284-1345).
+ * Per pixel, source bytes -> destination bytes:
+ *   RGB24_TO_BGRA       rgb_to_bgra          (r, g, b)    -> (b, g, r, 255)
+ *   RGBA_TO_BGRA        copy_swap_br         (r, g, b, a) -> (b, g, r, a); symmetric, so also BGRA -> RGBA
+ *   GRAY_TO_BGRA        gray_to_bgra         (v)          -> (v, v, v, 255)
+ *   GRAY_ALPHA_TO_BGRA  gray_alpha_to_bgra   (v, a)       -> (v, v, v, a)
+ *   BGRA_TO_RGB24       to_vec_rgb           (b, g, r, a) -> (r, g, b): alpha dropped, no matte
+ * opaque != 0 writes 255 into every alpha byte of a 4-byte output (the encoders' swap-then-fill-alpha, zen_encoder.rs:585-603, in one
+ * pass); BGRA_TO_RGB24 has none and ignores it.  Fill-alpha alone is IFB200_CANVAS_NORMALIZE_ALPHA.  RGBA_TO_BGRA may run in place
+ * (src == dst with the same stride: swap_br_inplace); any other overlap of the source and destination byte spans is refused.  Strides
+ * must hold a row; a 4-byte output needs a 4-byte aligned dst and dst_stride, while 1-, 2- and 3-byte rows may start at any byte.  A job
+ * of zero area is skipped unchecked.  Planar (CHW), 16-bit and indexed sources are not covered. */
+enum ifb200_pixel_op { IFB200_PIXEL_RGB24_TO_BGRA = 0, IFB200_PIXEL_RGBA_TO_BGRA = 1, IFB200_PIXEL_GRAY_TO_BGRA = 2,
+                       IFB200_PIXEL_GRAY_ALPHA_TO_BGRA = 3, IFB200_PIXEL_BGRA_TO_RGB24 = 4 };
+typedef struct ifb200_pixel_convert_desc {
+    int32_t        op;                      /* enum ifb200_pixel_op */
+    const uint8_t* src; uint32_t src_stride;   /* w x h source window; stride in bytes */
+    uint8_t*       dst; uint32_t dst_stride;   /* w x h destination window; may equal src for RGBA_TO_BGRA */
+    uint32_t       w, h;
+    int32_t        opaque;                  /* != 0: alpha = 255 in a 4-byte output */
+} ifb200_pixel_convert_desc;
+
 /* ---- device-resident batch API (the metric path; not in the reference) -----------------------
  * descs[i].in / .canvas are DEVICE pointers on the batch's device; color_matrix stays a HOST pointer.
  * enqueue is asynchronous on `cuda_stream`, a cudaStream_t with the usual CUDA meaning (NULL = the legacy
@@ -327,6 +350,12 @@ int  ifb200_batch_color_chain(ifb200_batch* b, const ifb200_color_desc* d, size_
  * skipped unchecked; every other descriptor is checked (as ifb200_batch_enqueue checks it, plus 4-byte aligned pointers and a NULL
  * colour matrix) and plans are built before anything is enqueued, so an error means nothing is written.  There is no host-buffer variant. */
 int  ifb200_batch_watermark(ifb200_batch* b, const ifb200_watermark_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
+/* Pixel-format conversions (ifb200_pixel_convert_desc) of n DEVICE windows in ONE kernel launch, none when no job has pixels; each
+ * destination byte is written once and nothing outside the two windows is read or written.  Asynchronous on `cuda_stream`.  No job may
+ * write what another job of the same call reads or writes (not checked).  Every descriptor is checked before anything is planned or
+ * enqueued, so an error means nothing is written.  There is no host-buffer variant: on host rows the decoders' own loop is cheaper than
+ * the trip over PCIe. */
+int  ifb200_batch_pixel_convert(ifb200_batch* b, const ifb200_pixel_convert_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
 int  ifb200_batch_sync(ifb200_batch* b, char* err, size_t err_cap);
 void ifb200_batch_destroy(ifb200_batch* b);
 /* knobs / introspection (benchmarks, tests) */

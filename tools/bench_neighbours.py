@@ -3,7 +3,8 @@
 and rounded corners; `bench_neighbours.py canvas` measures the canvas operations alone (canvas_rows), `bench_neighbours.py orient`
 the one-gather orientation against the reference's expansion into transposes and flips (orient_rows), `bench_neighbours.py color` the
 colour chains against the reference's node-by-node expansion (color_rows), `bench_neighbours.py watermark` the watermark composites
-against the node-by-node expansion and the best existing route (watermark_rows)
+against the node-by-node expansion and the best existing route (watermark_rows), `bench_neighbours.py formats` the pixel-format
+conversions against a torch copy of the same bytes and the torch expression a user would write (formats_rows)
 (the reference benchmarks transposes at 4K / 8K in benches/bench_graphics.rs:9-62).  Inputs resident in HBM, CUDA events on
 the launching stream, >= 3 warm-up calls; a set of 64 different images per size (>= 2 GB, far larger than L2) is cycled so that
 no call finds its data in cache.  One JSON line per (operation, size) with the HBM roofline of the kernel: algorithmic
@@ -593,6 +594,93 @@ def watermark_rows():
     b.sync()
 
 
+def formats_rows():
+    """Pixel-format conversions (Batch.pixel_convert) on rows resident in HBM: 64 3840x2160 frames in one call for each op, each timed
+    in five trials (median, smallest, largest) with the 64 frames (>= 1.6 GB) cycled, far larger than L2.  Algorithmic bytes per pixel:
+    7 for RGB24 <-> BGRA, 5 for Gray8, 6 for GrayAlpha8, 8 for RGBA <-> BGRA and the in-place swap.  Each row also times a torch
+    device-to-device copy of the same bytes and the torch expression a user would write today (a channel index, plus a cat with a
+    255 plane where the output gains an alpha), and checks frame 0 of the call against that expression, bit for bit.  Then 1024 512x384
+    RGB24 thumbnails in one call and as 1024 calls, with the CUDA-event time on the stream and the host wall time of the calls apart."""
+    card = _card()
+    pk, src = peak()
+    b = ifb.Batch(0)
+    stream = torch.cuda.current_stream().cuda_stream
+    n, w, h = 64, 3840, 2160
+    sbuf = torch.randint(0, 256, (n * h * w * 4,), dtype=torch.uint8, device="cuda")
+    dbuf = torch.empty(n * h * w * 4, dtype=torch.uint8, device="cuda")
+
+    def trials(fn, reps=10):
+        t = sorted(_time_ms(fn, reps) for _ in range(5))
+        return t[2], t[0], t[-1]
+
+    def full255(x):
+        return torch.full(x.shape[:-1] + (1,), 255, dtype=torch.uint8, device="cuda")
+
+    ops = [  # (row, record, source channels, destination channels, torch expression)
+        ("rgb24_to_bgra", ifb.RgbToBgra, 3, 4, lambda x: torch.cat([x[..., [2, 1, 0]], full255(x)], -1)),
+        ("rgba_to_bgra", ifb.RgbaToBgra, 4, 4, lambda x: x[..., [2, 1, 0, 3]]),
+        ("gray_to_bgra", ifb.GrayToBgra, 1, 4, lambda x: torch.cat([x[..., [0, 0, 0]], full255(x)], -1)),
+        ("gray_alpha_to_bgra", ifb.GrayAlphaToBgra, 2, 4, lambda x: x[..., [0, 0, 0, 1]]),
+        ("bgra_to_rgb24", ifb.BgraToRgb, 4, 3, lambda x: x[..., [2, 1, 0]]),
+    ]
+    for name, rec, cs, cd, expr in ops:
+        x = sbuf[:n * h * w * cs].view(n, h, w, cs)
+        y = dbuf[:n * h * w * cd].view(n, h, w, cd)
+        jobs = [rec(x[i], y[i]) for i in range(n)]
+        alg = n * w * h * (cs + cd)
+        ms, lo, hi = trials(lambda: b.pixel_convert(jobs, stream))
+        _, host = _time_event_and_host_ms(lambda: b.pixel_convert(jobs, stream), reps=3)
+        ms_torch, _, _ = trials(lambda: expr(x), reps=3)
+        b.pixel_convert(jobs[:1], stream)
+        ok = bool(torch.equal(y[0], expr(x[:1])[0]))
+        cm = _copy_ceiling_ms(alg)
+        print(json.dumps({"op": "formats", "row": f"{name}_64x{w}x{h}_one_call", "ms": ms, "ms_min": lo, "ms_max": hi,
+                          "host_wall_ms": host, "algorithmic_bytes": alg, "achieved_gbs": alg / ms / 1e6, "frac_of_peak": alg / ms / 1e6 / pk,
+                          "peak_gbs": pk, "peak_source": src, "torch_copy_same_bytes_ms": cm, "frac_of_torch_copy": cm / ms,
+                          "torch_expression_ms": ms_torch, "vs_torch_expression": ms_torch / ms, "bit_exact_vs_torch_expression": ok,
+                          **card}), flush=True)
+    # in place, opaque: the encoders' swap then fill-alpha in one pass
+    x = dbuf.view(n, h, w, 4)
+    x.copy_(sbuf.view(n, h, w, 4))
+    jobs = [ifb.RgbaToBgra(ifb.BitmapWindow.from_torch(x[i]), None, True) for i in range(n)]
+    alg = n * w * h * 8
+    ms, lo, hi = trials(lambda: b.pixel_convert(jobs, stream))
+
+    def torch_in_place(t):
+        t[..., :3] = t[..., [2, 1, 0]]
+        t[..., 3] = 255
+    ms_torch, _, _ = trials(lambda: torch_in_place(x), reps=3)
+    x.copy_(sbuf.view(n, h, w, 4))
+    b.pixel_convert(jobs[:1], stream)
+    want = sbuf.view(n, h, w, 4)[0].clone()
+    torch_in_place(want)
+    ok = bool(torch.equal(x[0], want))
+    cm = _copy_ceiling_ms(alg)
+    print(json.dumps({"op": "formats", "row": f"rgba_to_bgra_in_place_opaque_64x{w}x{h}_one_call", "ms": ms, "ms_min": lo, "ms_max": hi,
+                      "algorithmic_bytes": alg, "achieved_gbs": alg / ms / 1e6, "frac_of_peak": alg / ms / 1e6 / pk, "peak_gbs": pk,
+                      "peak_source": src, "torch_copy_same_bytes_ms": cm, "frac_of_torch_copy": cm / ms, "torch_expression_ms": ms_torch,
+                      "vs_torch_expression": ms_torch / ms, "bit_exact_vs_torch_expression": ok, **card}), flush=True)
+    del sbuf, dbuf, x, jobs
+    torch.cuda.empty_cache()
+
+    # thumbnails: 1024 x 512x384 RGB24 -> BGRA, one call and 1024 calls
+    n, w, h = 1024, 512, 384
+    ins = torch.randint(0, 256, (n, h, w, 3), dtype=torch.uint8, device="cuda")
+    outs = torch.empty((n, h, w, 4), dtype=torch.uint8, device="cuda")
+    jobs = [ifb.RgbToBgra(ins[i], outs[i]) for i in range(n)]
+    alg = n * w * h * 7
+    for label, fn, reps in (("one_call", lambda: b.pixel_convert(jobs, stream), 10),
+                            ("1024_calls", lambda: [b.pixel_convert([j], stream) for j in jobs], 3)):
+        t = sorted(_time_event_and_host_ms(fn, reps) for _ in range(5))
+        ev, host = t[2]
+        print(json.dumps({"op": "formats", "row": f"rgb24_to_bgra_1024x{w}x{h}_{label}", "ms": ev, "host_wall_ms": host,
+                          "algorithmic_bytes": alg, "achieved_gbs": alg / ev / 1e6, "frac_of_peak": alg / ev / 1e6 / pk, "peak_gbs": pk,
+                          "peak_source": src, "frames": n, **card}), flush=True)
+    ok = bool(torch.equal(outs[7], torch.cat([ins[7][..., [2, 1, 0]], full255(ins[7])], -1)))
+    print(json.dumps({"op": "formats", "row": "thumbnail_spot_check", "bit_exact_vs_torch_expression": ok, **card}))
+    b.sync()
+
+
 if __name__ == "__main__":
     if sys.argv[1:] == ["watermark"]:
         watermark_rows()
@@ -602,5 +690,7 @@ if __name__ == "__main__":
         orient_rows()
     elif sys.argv[1:] == ["color"]:
         color_rows()
+    elif sys.argv[1:] == ["formats"]:
+        formats_rows()
     else:
         main()
