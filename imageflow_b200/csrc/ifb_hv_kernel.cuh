@@ -232,6 +232,16 @@ __global__ void smem_base_probe_kernel(uint32_t* out) {
     if (threadIdx.x == 0) *out = hv::smem_u32(probe_smem);
 }
 
+// The LUT block's tables, filled by threads t, t + NT, ..: forward LUT replicated for the 32 lanes; linear->sRGB table into
+// holes 0..127.  Its own function so that tests/gpu_units gives hv_finish_pixel() the very layout the kernel reads.
+template <int NT>
+__device__ __forceinline__ void hv_fill_luts(const uint32_t lut, const Tables& tb, const uint32_t flags0, const int t) {
+    const float* __restrict__ T = (flags0 & JF_LINEAR) ? tb.t_lin : tb.t_srgb;
+    for (int i = t; i < 256 * 32; i += NT) hv::sts_f32(lut + ((uint32_t)(i >> 5) << 8) + ((uint32_t)(i & 31) << 2), hv::ldg(T + (i >> 5)));
+    const uint32_t* __restrict__ r32 = reinterpret_cast<const uint32_t*>(tb.lut16k);
+    for (int i = t; i < 4096; i += NT) hv::sts_u32(lut + 128u + (uint32_t)(i * 4) + ((uint32_t)(i * 4) & 0x3f80u), hv::ldg(r32 + i));
+}
+
 // Store epilogue with the tables in shared memory: same operations, same order as finish_pixel().
 //   enc(v)  floatspace_to_srgb (color.rs:59-69): linear -> 16 K table in the LUT holes; sRGB space -> uchar_clamp_ff(255 v)
 //   tl(b)   byte_to_float of the working space = the lane's own copy in the replicated LUT
@@ -319,13 +329,7 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
     const uint32_t flagw = sb + hv_flag_offset<AV, CH>(sb & 0xffffu);
     const uint32_t flags0 = jobs[0].flags;                                 // working space and channel count are the same for all jobs of a launch
 
-    // ---- tables: forward LUT replicated for the 32 lanes; linear->sRGB table into holes 0..127
-    {
-        const float* __restrict__ T = (flags0 & JF_LINEAR) ? tb.t_lin : tb.t_srgb;
-        for (int i = t; i < 256 * 32; i += C::kThreads) hv::sts_f32(lut + ((uint32_t)(i >> 5) << 8) + ((uint32_t)(i & 31) << 2), hv::ldg(T + (i >> 5)));
-        const uint32_t* __restrict__ r32 = reinterpret_cast<const uint32_t*>(tb.lut16k);
-        for (int i = t; i < 4096; i += C::kThreads) hv::sts_u32(lut + 128u + (uint32_t)(i * 4) + ((uint32_t)(i * 4) & 0x3f80u), hv::ldg(r32 + i));
-    }
+    hv_fill_luts<C::kThreads>(lut, tb, flags0, t);
     if (lane == 0) {
         for (int s = 0; s < S; ++s) hv::mbar_init(mb + 8u * s, 1u);
         hv::mbar_init_fence();

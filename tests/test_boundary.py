@@ -191,27 +191,6 @@ def test_descriptor_arrays_are_filled_in_place_like_single_descriptors():
         assert one == got, i
 
 
-def test_three_instruction_clamp_equals_uchar_clamp_ff_for_every_float(tmp_path):
-    """fused_tile2_kernel clamps with min(cvt.rzi.u32(add.rz(x, 0.5)), 255); tools/check_clamp_rz.c compares that with the
-    reference's uchar_clamp_ff (color.rs:101-108) on all 2^32 float bit patterns (a few seconds on the host cores)."""
-    exe = str(tmp_path / "check_clamp_rz")
-    src = os.path.join(ROOT, "tools", "check_clamp_rz.c")
-    subprocess.run(["gcc", "-O2", "-fopenmp", "-frounding-math", src, "-o", exe, "-lm"], check=True)
-    r = subprocess.run([exe], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0 and r.stdout.strip().endswith("0 mismatches over all 2^32 floats"), r.stdout[-500:]
-
-
-def test_shared_reciprocal_division_is_the_ieee_quotient(tmp_path):
-    """fused_tile2_kernel divides the three numerators of a composite by one correctly rounded reciprocal and a residual correction
-    each (t2_div3); tools/check_shared_reciprocal.c compares that with the IEEE quotient on random and near-midpoint operands inside
-    the kernel's guards (30 M trials per class here; 100 M per class were run for DESIGN.md section 5.2)."""
-    exe = str(tmp_path / "check_shared_reciprocal")
-    src = os.path.join(ROOT, "tools", "check_shared_reciprocal.c")
-    subprocess.run(["gcc", "-O2", "-ffp-contract=off", src, "-o", exe, "-lm"], check=True)
-    r = subprocess.run([exe, "30"], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0 and r.stdout.strip().endswith("mismatches 0"), r.stdout[-500:]
-
-
 def test_tile_kernel_float_quotients_are_exact():
     """fused_tile2_kernel starts a thread's items at (t / ic, t % ic) and advances by 256 / ic without an integer division:
     q = (int)((t + 0.5f) * (1.0f / ic)) and (int)(256.5f * (1.0f / ic)).  Exact for every t < 256 and every tile width."""
