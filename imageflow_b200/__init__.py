@@ -8,7 +8,9 @@ Host-side mirror of the reference seam (paths relative to the imageflow checkout
   graphics/blend.rs:6-59        apply_matte
   graphics/transpose.rs:95      bitmap_window_transpose;  graphics/flip.rs:10,25  flips
   flow/nodes/white_balance.rs   white_balance_srgb_mut (histogram.rs, area thresholds, byte maps)
-  graphics/whitespace.rs:284    detect_content (code map on the GPU, the reference's window walk on the host)
+  graphics/whitespace.rs:284    detect_content, the reference's window walk included, on the GPU for one frame or many at once
+      (Batch.detect_content_many), and the CropWhitespace node on top of it (Batch.crop_whitespace; RIAPI's trim.threshold /
+      trim.percentpadding as riapi_trim_steps); the code map and the host walk alone as Batch.whitespace_codes / detect_content_from_codes
   graphics/rounded_corners.rs:187  flow_bitmap_bgra_clear_around_rounded_corners, RoundCornersMode (imageflow_types)
   graphics/bitmaps.rs:1504,1570, graphics/copy_rect.rs:12  fill_rectangle, normalize_unused_alpha, copy_rectangle (Batch.canvas:
       FillRect, EnableTransparency, CopyRectToCanvas, ExpandCanvas; WatermarkRedDot, Region, RegionPercent as helpers)
@@ -35,7 +37,7 @@ from .graphics import (Batch, apply_matte, BitmapCompositing, BitmapWindow, Erro
                        riapi_flip_steps, apply_orientation, oriented_source_window, ColorMatrixSrgb, ColorFilterSrgb, WhiteBalanceHistogramAreaThresholdSrgb,
                        riapi_color_steps, Watermark, WatermarkConstraintBox, WatermarkConstraintMode, ConstraintGravity, WatermarkDraw,
                        process_constraint, watermark_layout, riapi_watermark_placement, PixelRows, RgbToBgra, RgbaToBgra, GrayToBgra,
-                       GrayAlphaToBgra, BgraToRgb, pixel_op_for)
+                       GrayAlphaToBgra, BgraToRgb, pixel_op_for, CropWhitespace, riapi_trim_steps, crop_whitespace_bounds)
 from ._lib import LIB_PATH, ResampleDesc, lib
 
 __all__ = [
@@ -49,5 +51,5 @@ __all__ = [
     "riapi_flip_steps", "apply_orientation", "oriented_source_window", "ColorMatrixSrgb", "ColorFilterSrgb", "WhiteBalanceHistogramAreaThresholdSrgb",
     "riapi_color_steps", "Watermark", "WatermarkConstraintBox", "WatermarkConstraintMode", "ConstraintGravity", "WatermarkDraw",
     "process_constraint", "watermark_layout", "riapi_watermark_placement", "PixelRows", "RgbToBgra", "RgbaToBgra", "GrayToBgra",
-    "GrayAlphaToBgra", "BgraToRgb", "pixel_op_for", "LIB_PATH", "ResampleDesc", "lib",
+    "GrayAlphaToBgra", "BgraToRgb", "pixel_op_for", "CropWhitespace", "riapi_trim_steps", "crop_whitespace_bounds", "LIB_PATH", "ResampleDesc", "lib",
 ]

@@ -22,7 +22,7 @@ SYMBOLS = [
     "ifb200_batch_fused_jobs", "ifb200_batch_generic_jobs", "ifb200_batch_tile_jobs", "ifb200_batch_ring_status", "ifb200_hv_plan_tables",
     "ifb200_block_scale_u8", "ifb200_batch_block_scale", "ifb200_round_corners_bgra8", "ifb200_batch_round_corners",
     "ifb200_batch_canvas", "ifb200_batch_orient", "ifb200_batch_color_chain", "ifb200_batch_watermark",
-    "ifb200_batch_pixel_convert", "ifb200_batch_enqueue_oriented",
+    "ifb200_batch_pixel_convert", "ifb200_batch_enqueue_oriented", "ifb200_batch_detect_content_many",
 ]
 
 
@@ -96,6 +96,12 @@ class PixelConvertDesc(C.Structure):
     ]
 
 
+class DetectContentDesc(C.Structure):
+    """struct ifb200_detect_content_desc"""
+    _fields_ = [("px", C.c_void_p), ("w", C.c_uint32), ("h", C.c_uint32), ("stride", C.c_uint32), ("alpha_meaningful", C.c_int32),
+                ("threshold", C.c_uint32)]
+
+
 _lib = None
 
 
@@ -150,7 +156,10 @@ def lib() -> C.CDLL:
     L.ifb200_batch_whitespace_codes.restype = C.c_int
     L.ifb200_detect_content_from_codes.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, u32p, C.POINTER(C.c_uint64)]
     L.ifb200_detect_content_from_codes.restype = C.c_int
-    L.ifb200_batch_white_balance.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, C.c_void_p, C.c_char_p, C.c_size_t]
+    L.ifb200_batch_detect_content_many.argtypes = [C.c_void_p, C.POINTER(DetectContentDesc), C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_char_p, C.c_size_t]
+    L.ifb200_batch_detect_content_many.restype = C.c_int
+    L.ifb200_batch_white_balance.argtypes =[C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_white_balance.restype = C.c_int
     L.ifb200_batch_transpose.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_transpose.restype = C.c_int

@@ -1231,26 +1231,62 @@ void whitespace_codes_locked(ifb200_batch* b, const uint8_t* px, uint32_t w, uin
     }
 }
 
-// detect_content (graphics/whitespace.rs:284-331) on a DEVICE bitmap: the per-pixel code map on the GPU, one byte per pixel
-// back to the host, the reference's window walk over it there.  Returns a rectangle, so it synchronises `st`.
+// detect_content of many DEVICE frames (ifb200_batch_detect_content_many, ifb_whitespace.h): every descriptor is checked before
+// anything is launched; then one upload of the plan, ONE launch of whitespace_segments_kernel over every frame of at least 3 x 3 and
+// ONE of whitespace_walk_kernel (none when no frame needs a walk), and one copy of the results back.  Synchronises `st`.
+void detect_content_many_locked(ifb200_batch* b, const ifb200_detect_content_desc* d, size_t n, uint32_t* rects, uint64_t* visited,
+                                cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    if (!rects && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null rectangle array");
+    ifb::WsWork wk;
+    int code = 0;
+    const std::string why = ifb::detect_content_prepare(d, n, wk, &code, nullptr, nullptr);
+    if (!why.empty()) IFB_THROW(code, "%s", why.c_str());
+    if (wk.ctas() > 0x7fffffffu || wk.jobs.size() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
+    std::vector<ifb::WsResult> res(wk.jobs.size());
+    if (!wk.jobs.empty()) {
+        DeviceScope dev_scope_(b->device);
+        const size_t res_bytes = res.size() * sizeof(ifb::WsResult);
+        WorkUpload up(b, st, {part(wk.jobs), part(wk.cols), part(wk.segs), part(wk.first)}, (size_t)wk.n_sums * 4 + 256 + res_bytes);
+        uint32_t* sums = up.at<uint32_t>(4);
+        ifb::WsResult* dres = reinterpret_cast<ifb::WsResult*>(reinterpret_cast<uint8_t*>(sums) + ((size_t)wk.n_sums * 4 + 255) / 256 * 256);
+        if (wk.ctas()) {
+            whitespace_segments_kernel<<<(unsigned)wk.ctas(), dim3(ifb::kWsChunk, ifb::kWsBand), 0, st>>>(
+                up.at<const ifb::WsSeg>(2), up.at<const uint32_t>(3), (uint32_t)wk.segs.size(), sums);
+            CUDA_OK(cudaGetLastError());
+            b->launches++;
+        }
+        whitespace_walk_kernel<<<(unsigned)wk.jobs.size(), 32, 0, st>>>(up.at<const ifb::WsJob>(0), up.at<const ifb::WsColumn>(1), sums, dres);
+        CUDA_OK(cudaGetLastError());
+        b->launches++;
+        cudaEvent_t ev;
+        ifb::WsResult* host = static_cast<ifb::WsResult*>(b->stage(res_bytes, &ev));
+        CUDA_OK(cudaMemcpyAsync(host, dres, res_bytes, cudaMemcpyDeviceToHost, st));
+        CUDA_OK(cudaEventRecord(ev, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        memcpy(res.data(), host, res_bytes);
+    }
+    for (size_t k = 0; k < res.size(); ++k)
+        if (res[k].bad) IFB_THROW(IFB200_ERR_INVALID_STATE, "detect_content job %u: the window walk met a window it cannot replay", wk.job_of[k]);
+    for (size_t i = 0; i < n; ++i) {
+        rects[4 * i] = 0; rects[4 * i + 1] = 0; rects[4 * i + 2] = d[i].w; rects[4 * i + 3] = d[i].h;       // whitespace.rs:288-290
+        if (visited) visited[i] = 0;
+    }
+    for (size_t k = 0; k < res.size(); ++k) {
+        const uint32_t i = wk.job_of[k];
+        for (int q = 0; q < 4; ++q) rects[4 * i + q] = res[k].rect[q];
+        if (visited) visited[i] = res[k].visited;
+    }
+}
+
+// detect_content (graphics/whitespace.rs:284-331) of one DEVICE bitmap: a one-frame call of detect_content_many_locked, after the
+// checks and messages this entry point has always had.  Returns a rectangle, so it synchronises `st`.
 void detect_content_locked(ifb200_batch* b, const uint8_t* px, uint32_t w, uint32_t h, uint32_t stride, int alpha_meaningful,
                            uint32_t threshold, cudaStream_t st, uint32_t rect[4]) {
     if (!rect) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null pointer");
     whitespace_check(px, w, h, stride, threshold);
-    rect[0] = 0; rect[1] = 0; rect[2] = w; rect[3] = h;
-    if (w < 3 || h < 3) return;                              // whitespace.rs:288-290
-    DeviceScope dev_scope_(b->device);
-    const size_t n = (size_t)w * h;
-    cudaEvent_t ev;
-    uint8_t* codes = static_cast<uint8_t*>(b->stage(n, &ev));          // before any device allocation: may throw
-    uint8_t* dcodes = nullptr;
-    CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&dcodes), n, st));
-    AsyncFree dcodes_guard{dcodes, st};
-    whitespace_codes_locked(b, px, w, h, stride, alpha_meaningful, threshold, dcodes, st);
-    CUDA_OK(cudaMemcpyAsync(codes, dcodes, n, cudaMemcpyDeviceToHost, st));
-    CUDA_OK(cudaEventRecord(ev, st));
-    CUDA_OK(cudaStreamSynchronize(st));
-    if (!ifb::detect_content_from_codes(codes, w, h, rect, nullptr)) IFB_THROW(IFB200_ERR_INVALID_STATE, "whitespace walk failed");
+    const ifb200_detect_content_desc d{px, w, h, stride, alpha_meaningful ? 1 : 0, threshold};
+    detect_content_many_locked(b, &d, 1, rect, nullptr, st);
 }
 
 // ONE launch of round_corners_kernel for every tile of `wk`, asynchronous on `st` (none when no job touches a pixel)
@@ -2088,6 +2124,11 @@ int ifb200_detect_content_from_codes(const uint8_t* codes, uint32_t w, uint32_t 
 int ifb200_batch_detect_content(ifb200_batch* b, const uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, int alpha_meaningful,
                                 uint32_t threshold, uint32_t rect[4], void* stream, char* err, size_t cap) {
     return with_batch(b, stream, err, cap, [&](cudaStream_t st) { detect_content_locked(b, dev_px, w, h, stride, alpha_meaningful, threshold, st, rect); });
+}
+
+int ifb200_batch_detect_content_many(ifb200_batch* b, const ifb200_detect_content_desc* d, size_t n, uint32_t* rects, uint64_t* visited,
+                                     void* stream, char* err, size_t cap) {
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { detect_content_many_locked(b, d, n, rects, visited, st); });
 }
 
 int ifb200_batch_whitespace_codes(ifb200_batch* b, const uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, int alpha_meaningful,

@@ -24,6 +24,7 @@
 #include "ifb_color.h"             // ClJob / ClSeg: planned on the host, read by the colour-chain kernels
 #include "ifb_watermark.h"         // WmJob / WmGroup: planned on the host, read by watermark_composite_kernel
 #include "ifb_pixel_convert.h"     // PcItem: planned on the host, read by pixel_convert_kernel
+#include "ifb_whitespace.h"        // WsSeg / WsJob / WsColumn: planned on the host, read by the detect_content_many kernels
 
 namespace ifbk {
 

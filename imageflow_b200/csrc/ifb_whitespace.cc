@@ -4,12 +4,16 @@
 // floor(1.0 * (w - 1)) (whitespace.rs:221-236), windows of at most 2048 grayscale bytes overlap by two, and every window is
 // skipped, shrunk or moved according to the bounding box found so far (:352-408).  The bounding box of all codes is an outer
 // bound of the result and differs from it on about one image in seven (measured in the tests), so the walk is
-// reproduced step by step; only the arithmetic per pixel -- grayscale, Scharr, the local edge box -- runs on the GPU.
+// reproduced step by step.  detect_content_from_codes is that walk over a code map, on the host (the public
+// ifb200_detect_content_from_codes, and the reference the tests hold the device walk to); whitespace_grid / detect_content_prepare
+// plan the device walk of ifb200_batch_detect_content_many (ifb_whitespace.h, DESIGN.md §5.16).
 #include "ifb_whitespace.h"
 
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+
+#include "ifb_prepare.h"
 
 namespace ifb {
 namespace {
@@ -116,6 +120,71 @@ bool detect_content_from_codes(const uint8_t* codes, uint32_t w, uint32_t h, uin
     if (!(k.lo_x == w && k.hi_x == 0 && k.lo_y == h && k.hi_y == 0)) { rect[0] = k.lo_x; rect[1] = k.lo_y; rect[2] = k.hi_x; rect[3] = k.hi_y; }
     if (centres) *centres = k.visited;
     return true;
+}
+
+void whitespace_grid(uint32_t w, uint32_t h, WsJob& job, std::vector<WsColumn>& cols) {
+    job.rows = 0; job.ncols = 0;
+    const Walk k{nullptr, w, h, w, 0, h, 0};
+    const Walk::Box s = k.search_rect(kFull);                // the full scan reads no box (Edge::None)
+    if (!s.any) return;
+    // Walk::region's arithmetic, for the full scan
+    const uint32_t rw = s.x2 - s.x1, rh = s.y2 - s.y1;
+    const uint32_t ww = std::min(rw, kBuffer / 7u), wh = std::min(rh, kBuffer / ww);
+    if (ww <= 2 || wh <= 2) return;
+    job.y1 = s.y1; job.y2 = s.y2; job.wh = wh;
+    job.rows = (uint32_t)std::ceil((float)rh / (float)(wh - 2));
+    job.ncols = (uint32_t)std::ceil((float)rw / (float)(ww - 2));
+    for (uint32_t i = 0; i < job.ncols; ++i) {
+        uint32_t bx = s.x1 + (ww - 2) * i, bw = std::min(std::max(3u, s.x2 - bx), ww);
+        WsColumn c{bx, bx + bw, 0, 0, 0, 0};
+        if (bx + bw > w) { if (bw <= w) bx = w - bw; else { bx = 0; bw = w; } }
+        c.xa = bx + 1; c.xb = std::max(bx + 1, bx + bw - 1);
+        cols.push_back(c);
+    }
+}
+
+std::string detect_content_check(const ifb200_detect_content_desc& d, int* code) {
+    if (code) *code = IFB200_ERR_INVALID_ARGUMENT;
+    // whitespace_check's limits and messages (ifb_engine.cu), plus the alignment of the kernels' 4-byte pixel loads
+    if (!d.px) return "null bitmap pointer";
+    if (d.w == 0 || d.h == 0) return "empty bitmap";
+    if (d.stride < d.w * 4ull || (d.stride & 3)) return "stride smaller than a BGRA row or not a multiple of 4";
+    if (reinterpret_cast<uintptr_t>(d.px) & 3) return "bitmap pointer not 4-byte aligned";
+    if (d.w > 0x7fffffffu || d.h > 0x7fffffffu) return "oversized bitmap";
+    if (d.threshold > 0x7fffffffu) return "threshold out of range";
+    return "";
+}
+
+std::string detect_content_prepare(const ifb200_detect_content_desc* d, size_t n, WsWork& wk, int* code, uint32_t* rects, uint64_t* visited) {
+    const std::string why = check_each("detect_content", d, n, detect_content_check, code);
+    if (!why.empty()) return why;
+    for (size_t i = 0; i < n; ++i) {
+        if (rects) { rects[4 * i] = 0; rects[4 * i + 1] = 0; rects[4 * i + 2] = d[i].w; rects[4 * i + 3] = d[i].h; }
+        if (visited) visited[i] = 0;
+        if (d[i].w < 3 || d[i].h < 3) continue;              // whitespace.rs:288-290
+        WsJob job{};
+        job.w = d[i].w; job.h = d[i].h; job.col0 = (uint32_t)wk.cols.size();
+        whitespace_grid(job.w, job.h, job, wk.cols);
+        job.sum0 = wk.n_sums;
+        const uint64_t bands = (job.h + kWsBand - 1) / kWsBand;
+        for (uint32_t c = job.col0; c < job.col0 + job.ncols; ++c) {
+            WsColumn& col = wk.cols[c];
+            col.chunk0 = job.tch; col.nch = (col.xb - col.xa + kWsChunk - 1) / kWsChunk;
+            job.tch += col.nch;
+        }
+        for (uint32_t c = job.col0; c < job.col0 + job.ncols; ++c) {
+            const WsColumn& col = wk.cols[c];
+            if (col.nch == 0) continue;
+            wk.segs.push_back({d[i].px, job.w, job.h, d[i].stride, d[i].alpha_meaningful ? 1u : 0u, (int32_t)d[i].threshold, col.xa, col.xb,
+                               col.chunk0, col.nch, job.tch, job.sum0});
+            if (wk.first.empty()) wk.first.push_back(0);
+            wk.first.push_back((uint32_t)std::min<uint64_t>(wk.first.back() + bands * col.nch, 0xffffffffull));
+        }
+        wk.n_sums += (uint64_t)job.h * job.tch;
+        wk.jobs.push_back(job);
+        wk.job_of.push_back((uint32_t)i);
+    }
+    return "";
 }
 
 }  // namespace ifb

@@ -9,7 +9,7 @@ from typing import Optional, Sequence
 
 import numpy as np
 
-from ._lib import (CanvasDesc, ColorDesc, ColorStep, OrientDesc, OrientedResampleDesc, PixelConvertDesc, ResampleDesc, RoundCornersDesc,
+from ._lib import (CanvasDesc, ColorDesc, ColorStep, DetectContentDesc, OrientDesc, OrientedResampleDesc, PixelConvertDesc, ResampleDesc, RoundCornersDesc,
                    WatermarkDesc, lib)
 
 
@@ -940,6 +940,55 @@ def detect_content_from_codes(codes: np.ndarray):
     return tuple(rect), n.value
 
 
+@dataclass(frozen=True)
+class CropWhitespace:
+    """Node::CropWhitespace { threshold, percent_padding } (flow/nodes/clone_crop_fill_expand.rs:557-628): detect_content of the frame,
+    the rectangle grown by a padding of percent_padding % of its mean side, clamped to the frame, then a crop (Batch.crop_whitespace)."""
+    threshold: int
+    percent_padding: float = 0.0
+
+
+def riapi_trim_steps(threshold=None, percentpadding=None) -> list:
+    """The step RIAPI's layout adds right after decoding for trim.threshold / trim.percentpadding (imageflow_riapi ir4/mod.rs:107-111):
+    none without a threshold, else CropWhitespace(max(0, threshold), percentpadding or 0)."""
+    if threshold is None:
+        return []
+    return [CropWhitespace(max(0, int(threshold)), float(np.float32(0.0 if percentpadding is None else percentpadding)))]
+
+
+def _wrap_i64(v: int) -> int:
+    return (v + (1 << 63)) % (1 << 64) - (1 << 63)
+
+
+def _f32_to_i64_saturating(f: np.float32) -> int:
+    """Rust's `f32 as i64`: NaN -> 0, out of range -> i64::MIN / i64::MAX"""
+    if f != f:
+        return 0
+    if f >= np.float32(9.223372e18):
+        return (1 << 63) - 1
+    if f <= np.float32(-9.223372e18):
+        return -(1 << 63)
+    return int(f)
+
+
+def crop_whitespace_bounds(rect, w: int, h: int, percent_padding: float):
+    """CropWhitespaceDef::expand's arithmetic (clone_crop_fill_expand.rs:585-605) on the rectangle detect_content returned for a w x h
+    frame, then Bitmap::crop's check (bitmaps.rs:841-851) -> (x1, y1, x2, y2) of the crop.  Raises FlowError(InvalidState) for an
+    empty rectangle and FlowError(InvalidArgument) for an empty or out-of-frame crop (a negative padding can make one)."""
+    x1, y1, x2, y2 = (int(v) for v in rect)
+    if x2 <= x1 or y2 <= y1:
+        raise FlowError(ErrorKind.InvalidState, "Whitespace detection returned invalid rectangle")
+    side = np.float32(((x2 - x1) + (y2 - y1)) & 0xffffffff)                    # u32 sum as f32
+    with np.errstate(all="ignore"):
+        p = np.ceil(np.float32(np.float32(percent_padding) / np.float32(100.0)) * side / np.float32(2.0), dtype=np.float32)
+    pad = _f32_to_i64_saturating(np.float32(p))
+    c = (max(0, _wrap_i64(x1 - pad)) & 0xffffffff, max(0, _wrap_i64(y1 - pad)) & 0xffffffff,
+         min(w, _wrap_i64(x2 + pad)) & 0xffffffff, min(h, _wrap_i64(y2 + pad)) & 0xffffffff)
+    if c[2] <= c[0] or c[3] <= c[1] or c[2] > w or c[3] > h:
+        raise FlowError(ErrorKind.InvalidArgument, f"Invalid crop bounds (({c[0]}, {c[1]}), ({c[2]}, {c[3]})) (image {w}x{h})")
+    return c
+
+
 def color_filter_matrix(which: int, p: float = 0.0) -> np.ndarray:
     """flow/nodes/color.rs:86-225 presets (0 sepia ... 9 saturation)."""
     m = np.zeros(25, np.float32)
@@ -1210,6 +1259,43 @@ class Batch:
         _check(lib().ifb200_batch_detect_content(self._h, bitmap.ptr, bitmap.w, bitmap.h, bitmap.stride, int(bool(bitmap.alpha_meaningful)),
                                                  int(threshold), rect, self._stream(stream), buf, 512), buf)
         return tuple(rect)
+
+    def detect_content_many(self, jobs, visited: bool = False, stream=None):
+        """graphics/whitespace.rs:284-331 on many DEVICE frames in one call (two kernel launches, one copy back; synchronises `stream`).
+        jobs: iterable of (BitmapWindow, threshold).  -> [(x1, y1, x2, y2)] per frame, each what detect_content returns for it; with
+        visited, ([rects], [window-interior pixels the walk visited])."""
+        jobs = list(jobs)
+        arr = (DetectContentDesc * len(jobs))()
+        for d, (win, thr) in zip(arr, jobs):
+            if win.pixel_layout != "BGRA":
+                raise FlowError(ErrorKind.InvalidArgument, "Only BGRA supported for whitespace detection")
+            d.px, d.w, d.h, d.stride = win.ptr, win.w, win.h, win.stride
+            d.alpha_meaningful = int(bool(win.alpha_meaningful))
+            d.threshold = int(thr) if 0 <= int(thr) <= 0xffffffff else 0xffffffff      # out of range: rejected by the library
+        rects = np.zeros((len(jobs), 4), np.uint32)
+        counts = np.zeros(len(jobs), np.uint64)
+        buf = C.create_string_buffer(512)
+        _check(lib().ifb200_batch_detect_content_many(self._h, arr, len(jobs), rects.ctypes.data, counts.ctypes.data if visited else None,
+                                                      self._stream(stream), buf, 512), buf)
+        out = [tuple(int(v) for v in r) for r in rects]
+        return (out, [int(v) for v in counts]) if visited else out
+
+    def crop_whitespace(self, jobs, stream=None) -> list:
+        """CropWhitespace (flow/nodes/clone_crop_fill_expand.rs:557-628) of many DEVICE frames: one detect_content_many call, then the
+        node's padding, clamps and crop.  jobs: iterable of (BitmapWindow, CropWhitespace).  Returns the cropped windows: views into
+        the frames, nothing is copied.  A frame whose detected rectangle is empty raises FlowError(InvalidState), a crop that padding
+        makes empty FlowError(InvalidArgument); the message names the job."""
+        jobs = list(jobs)
+        rects = self.detect_content_many([(win, node.threshold) for win, node in jobs], stream=stream)
+        out = []
+        for i, ((win, node), rect) in enumerate(zip(jobs, rects)):
+            try:
+                x1, y1, x2, y2 = crop_whitespace_bounds(rect, win.w, win.h, node.percent_padding)
+            except FlowError as e:
+                raise FlowError(e.code, f"crop_whitespace job {i}: {str(e).split(': ', 1)[1]}") from None
+            out.append(BitmapWindow(win.ptr + y1 * win.stride + x1 * 4, x2 - x1, y2 - y1, win.stride, win.alpha_meaningful,
+                                    win.compose, win.matte_bgra, win.pixel_layout, win._keep))
+        return out
 
     def whitespace_codes(self, bitmap: BitmapWindow, dev_codes_ptr: int, threshold: int = 1, stream=None) -> None:
         """the GPU half of detect_content alone (graphics/whitespace.rs:426-613 per pixel): code map of a DEVICE bitmap into a

@@ -293,6 +293,16 @@ typedef struct ifb200_pixel_convert_desc {
     int32_t        opaque;                  /* != 0: alpha = 255 in a 4-byte output */
 } ifb200_pixel_convert_desc;
 
+/* One frame of ifb200_batch_detect_content_many: detect_content (graphics/whitespace.rs:284-331) of the DEVICE BGRA window px
+ * (w x h, row pitch `stride` bytes), grayscale Bgra32 when alpha_meaningful != 0 else Bgr32, edges where the Scharr value exceeds
+ * `threshold`.  The limits are those of ifb200_batch_detect_content: a non-empty window, w and h below 2^31, threshold below 2^31. */
+typedef struct ifb200_detect_content_desc {
+    const uint8_t* px;
+    uint32_t w, h, stride;
+    int32_t  alpha_meaningful;
+    uint32_t threshold;
+} ifb200_detect_content_desc;
+
 /* ---- device-resident batch API (the metric path; not in the reference) -----------------------
  * descs[i].in / .canvas are DEVICE pointers on the batch's device; color_matrix stays a HOST pointer.
  * enqueue is asynchronous on `cuda_stream`, a cudaStream_t with the usual CUDA meaning (NULL = the legacy
@@ -329,8 +339,8 @@ int  ifb200_batch_white_balance(ifb200_batch* b, uint8_t* dev_px, uint32_t w, ui
                                 void* cuda_stream, char* err, size_t err_cap);
 /* graphics/whitespace.rs:284-331 detect_content(&BitmapWindowMut<u8>, threshold) -> RectCorners{x1, y1, x2, y2}: the rectangle the
  * reference's whitespace scan finds (trim / `trim.threshold`).  The per-pixel arithmetic (approximate_grayscale :426-523, Scharr
- * and the local edge box :525-613) runs on the GPU for all pixels; the reference's order-dependent window walk (:333-421) is
- * replayed on the host over that one-byte-per-pixel map, so the result is the reference's, not the bounding box of all edges.
+ * and the local edge box :525-613) and the reference's order-dependent window walk (:333-421) both run on the GPU: this is a one-frame
+ * call of ifb200_batch_detect_content_many, so the result is the reference's, not the bounding box of all edges.
  * alpha_meaningful selects the Bgra32 (1) or Bgr32 (0) grayscale.  Synchronous (a rectangle comes back). */
 int  ifb200_batch_detect_content(ifb200_batch* b, const uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, int alpha_meaningful,
                                  uint32_t threshold, uint32_t rect[4], void* cuda_stream, char* err, size_t err_cap);
@@ -339,6 +349,16 @@ int  ifb200_batch_detect_content(ifb200_batch* b, const uint8_t* dev_px, uint32_
  * Asynchronous on `cuda_stream`; ifb200_detect_content_from_codes() walks a host copy of it. */
 int  ifb200_batch_whitespace_codes(ifb200_batch* b, const uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, int alpha_meaningful,
                                    uint32_t threshold, uint8_t* dev_codes, void* cuda_stream, char* err, size_t err_cap);
+/* detect_content of n DEVICE frames (ifb200_detect_content_desc) in one call: rects[4 i .. 4 i + 3] (HOST memory) = {x1, y1, x2, y2}
+ * of frame i, exactly what ifb200_batch_detect_content returns for it; visited (HOST, may be NULL) = the walk's count of
+ * window-interior pixels, as ifb200_detect_content_from_codes reports it.  No code map is written: whitespace_segments_kernel reduces
+ * every frame's codes into one summary per (interior row, 32-column chunk of a window column), and whitespace_walk_kernel replays the
+ * reference's window order over those summaries on the device, one warp per frame (DESIGN.md §5.16).  Two kernel launches per call
+ * whatever n is, none when no frame is at least 3 x 3 (those get the whole bitmap without any device work), and one device-to-host
+ * copy of the results.  Every descriptor is checked before anything is launched ("detect_content job i: <why>").  Synchronous:
+ * `cuda_stream` is synchronised before the call returns. */
+int  ifb200_batch_detect_content_many(ifb200_batch* b, const ifb200_detect_content_desc* d, size_t n, uint32_t* rects, uint64_t* visited,
+                                      void* cuda_stream, char* err, size_t err_cap);
 /* Rounded corners of n DEVICE windows (d[i].px on the batch's device) in ONE kernel launch, asynchronous on `cuda_stream`.  The jobs
  * of one call must not overlap in memory (no two windows may share a pixel): they run concurrently.  Argument errors are reported
  * before anything is enqueued. */

@@ -4,7 +4,8 @@ and rounded corners; `bench_neighbours.py canvas` measures the canvas operations
 the one-gather orientation against the reference's expansion into transposes and flips (orient_rows), `bench_neighbours.py color` the
 colour chains against the reference's node-by-node expansion (color_rows), `bench_neighbours.py watermark` the watermark composites
 against the node-by-node expansion and the best existing route (watermark_rows), `bench_neighbours.py formats` the pixel-format
-conversions against a torch copy of the same bytes and the torch expression a user would write (formats_rows)
+conversions against a torch copy of the same bytes and the torch expression a user would write (formats_rows), `bench_neighbours.py
+trim` the batched whitespace trim against per-frame detect_content and the host walk (trim_rows; `trim_profile` its kernel times)
 (the reference benchmarks transposes at 4K / 8K in benches/bench_graphics.rs:9-62).  Inputs resident in HBM, CUDA events on
 the launching stream, >= 3 warm-up calls; a set of 64 different images per size (>= 2 GB, far larger than L2) is cycled so that
 no call finds its data in cache.  One JSON line per (operation, size) with the HBM roofline of the kernel: algorithmic
@@ -681,8 +682,95 @@ def formats_rows():
     b.sync()
 
 
+def _shots(n, w, h, seed):
+    """n product shots on the GPU: white BGRA frames (rows padded to 64 bytes) each with a noisy photo rectangle at a random place"""
+    g = torch.Generator(device="cuda"); g.manual_seed(seed)
+    rng = np.random.default_rng(seed)
+    pitch = (w * 4 + 63) // 64 * 64
+    out = []
+    for _ in range(n):
+        t = torch.full((h, pitch // 4, 4), 255, dtype=torch.uint8, device="cuda")
+        x1, y1 = int(rng.integers(w // 20, w // 4)), int(rng.integers(h // 20, h // 4))
+        x2, y2 = int(rng.integers(w * 3 // 4, w - w // 20)), int(rng.integers(h * 3 // 4, h - h // 20))
+        t[y1:y2, x1:x2] = torch.randint(0, 256, (y2 - y1, x2 - x1, 4), dtype=torch.uint8, device="cuda", generator=g)
+        out.append(ifb.BitmapWindow.from_torch(t[:, :w], alpha_meaningful=True))
+    return out
+
+
+def trim_rows(profile=False):
+    """Whitespace trim (Batch.detect_content_many / crop_whitespace) of frames resident in HBM, each route timed in five trials of one
+    synchronous call (median, smallest, largest, host wall clock).  (a) 64 3840x2160 product shots at threshold 80: the batched call,
+    64 calls of Batch.detect_content, and the host walk alone over the 64 code maps; (b) 1024 512x512 shots; (c) trim-then-resize: the
+    batched crop, then scale_and_render_many of the cropped windows to 450x450; (d) one 3840x2160 frame through both entry points.
+    Algorithmic bytes: 4 per pixel.  With profile=True, the kernels' own times from torch.profiler instead (a run of its own)."""
+    card = _card()
+    b = ifb.Batch(0)
+    st = torch.cuda.current_stream().cuda_stream
+
+    def trials(fn, reps=5):
+        fn(); torch.cuda.synchronize()
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter(); fn(); torch.cuda.synchronize(); ts.append((time.perf_counter() - t0) * 1e3)
+        return float(np.median(ts)), min(ts), max(ts)
+
+    def row(name, fn, px, **kw):
+        if profile:
+            from torch.profiler import ProfilerActivity, profile as prof_
+            fn(); torch.cuda.synchronize()
+            with prof_(activities=[ProfilerActivity.CUDA]) as p:
+                for _ in range(5):
+                    fn()
+                torch.cuda.synchronize()
+            kern = {e.key: (getattr(e, "self_device_time_total", None) or getattr(e, "self_cuda_time_total", 0)) / 1e3 / 5
+                    for e in p.key_averages() if (getattr(e, "self_device_time_total", None) or getattr(e, "self_cuda_time_total", 0)) > 0}
+            seg = sum(v for k, v in kern.items() if "segments" in k)
+            print(json.dumps({"op": "trim", "row": name, "profile_ms_per_call": {k[:60]: round(v, 4) for k, v in kern.items()},
+                              "segments_GBps": round(px * 4 / seg / 1e6, 1) if seg else None, **card}))
+            return
+        ms, lo, hi = trials(fn)
+        print(json.dumps({"op": "trim", "row": name, "ms": round(ms, 3), "ms_min": round(lo, 3), "ms_max": round(hi, 3),
+                          "alg_GBps": round(px * 4 / ms / 1e6, 1), **kw, **card}))
+
+    for n, w, h in ((64, 3840, 2160), (1024, 512, 512)):
+        wins = _shots(n, w, h, 5 + n)
+        px = n * w * h
+        one = lambda: b.detect_content_many([(x, 80) for x in wins], stream=st)
+        per = lambda: [b.detect_content(x, 80, stream=st) for x in wins]
+        same = one() == per()
+        row(f"detect_content_many_{n}x{w}x{h}", one, px, bit_exact_vs_per_frame=same)
+        row(f"detect_content_per_frame_{n}x{w}x{h}", per, px)
+        if n == 64 and not profile:
+            maps = []
+            for x in wins:
+                d = torch.empty((h, w), dtype=torch.uint8, device="cuda")
+                b.whitespace_codes(x, d.data_ptr(), 80, stream=st)
+                maps.append(d.cpu().numpy())
+            walk = lambda: [ifb.detect_content_from_codes(m) for m in maps]
+            ms, lo, hi = trials(walk)
+            print(json.dumps({"op": "trim", "row": f"host_walk_alone_{n}x{w}x{h}", "ms": round(ms, 3), "ms_min": round(lo, 3),
+                              "ms_max": round(hi, 3), **card}))
+            del maps
+        if n == 64:
+            outs = [ifb.new_canvas(450, 450) for _ in range(n)]
+
+            def trim_resize():
+                crops = b.crop_whitespace([(x, ifb.CropWhitespace(80, 0.5)) for x in wins], stream=st)
+                b.scale_and_render_many([(c, o, ifb.ScaleAndRenderParams(w=450, h=450)) for c, o in zip(crops, outs)], stream=st)
+            row(f"trim_then_resize_450x450_{n}x{w}x{h}", trim_resize, px)
+            row(f"detect_content_many_1x{w}x{h}", lambda: b.detect_content_many([(wins[0], 80)], stream=st), w * h)
+            row(f"detect_content_single_1x{w}x{h}", lambda: b.detect_content(wins[0], 80, stream=st), w * h)
+        del wins
+        torch.cuda.empty_cache()
+    b.sync()
+
+
 if __name__ == "__main__":
-    if sys.argv[1:] == ["watermark"]:
+    if sys.argv[1:] == ["trim"]:
+        trim_rows()
+    elif sys.argv[1:] == ["trim_profile"]:
+        trim_rows(profile=True)
+    elif sys.argv[1:] == ["watermark"]:
         watermark_rows()
     elif sys.argv[1:] == ["canvas"]:
         canvas_rows()
