@@ -485,7 +485,7 @@ struct ifb200_batch {
     // counters
     uint64_t launches = 0, fused_jobs = 0, generic_jobs = 0, tile_jobs = 0;
     // where the calling thread spends an enqueue (seconds, inclusive; ifb200_batch_host_profile)
-    struct { double enqueue = 0, plans = 0, stage = 0, memcpy_ = 0, upload = 0; uint64_t commits = 0, staged_bytes = 0, pinned_allocs = 0; } prof;
+    struct { double enqueue = 0, plans = 0, stage = 0, memcpy_ = 0, upload = 0; uint64_t commits = 0, staged_bytes = 0, pinned_allocs = 0, ring_bands = 0; } prof;
 
     ~ifb200_batch() {
         cudaSetDevice(device);
@@ -997,6 +997,7 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
             CUDA_OK(cudaGetLastError());
             b->launches++;
             b->fused_jobs += nj;
+            b->prof.ring_bands += (uint64_t)lay[gi].nb;
         } else {
             // generic pair; the float4 intermediate [in_h][out_w] is bounded to ~1 GiB per chunk of jobs
             const size_t per = (size_t)p.in_h * p.out_w * sizeof(float4);
@@ -1947,10 +1948,10 @@ int ifb200_batch_set_option(ifb200_batch* b, int option, int64_t value) {
 }
 int ifb200_batch_host_profile(const ifb200_batch* b, double* out, int n) {
     if (!b) return 0;
-    const double v[8] = {b->prof.enqueue, b->prof.plans, b->prof.stage, b->prof.memcpy_, b->prof.upload,
-                         (double)b->prof.commits, (double)b->prof.staged_bytes, (double)b->prof.pinned_allocs};
-    for (int i = 0; i < n && i < 8; ++i) if (out) out[i] = v[i];
-    return 8;
+    const double v[9] = {b->prof.enqueue, b->prof.plans, b->prof.stage, b->prof.memcpy_, b->prof.upload,
+                         (double)b->prof.commits, (double)b->prof.staged_bytes, (double)b->prof.pinned_allocs, (double)b->prof.ring_bands};
+    for (int i = 0; i < n && i < 9; ++i) if (out) out[i] = v[i];
+    return 9;
 }
 uint64_t ifb200_batch_kernel_launches(const ifb200_batch* b) { return b ? b->launches : 0; }
 uint64_t ifb200_batch_fused_jobs(const ifb200_batch* b) { return b ? b->fused_jobs : 0; }

@@ -140,8 +140,12 @@ __global__ void __launch_bounds__(256) color_matrix_kernel(uint8_t* __restrict__
     __shared__ float m[20];
     if (threadIdx.x < 20) m[threadIdx.x] = m20[threadIdx.x];
     __syncthreads();
-    const uint32_t total = w * h;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    // The thread's pixels are counted before the loop: on a frame of more than 2^32 - step pixels (the host bounds w * h to
+    // 2^32 - 1), `i < total` after a wrapping `i += step` would hold again and start another pass over finished pixels.
+    const uint32_t total = w * h, step = gridDim.x * blockDim.x, first = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t n = first < total ? (total - 1u - first) / step + 1u : 0u;
+    uint32_t i = first;
+    for (uint32_t k = 0; k < n; ++k, i += step) {
         const uint32_t y = i / w, x = i - y * w;
         uint32_t* p = reinterpret_cast<uint32_t*>(px + (size_t)y * stride) + x;
         const uint32_t v = *p;
@@ -166,8 +170,10 @@ __global__ void __launch_bounds__(256) apply_matte_kernel(uint8_t* __restrict__ 
     const float a2f = 1.0f / 255.0f;
     const float ma = __fmul_rn((float)(matte_bgra >> 24), a2f);
     const float mb = __ldg(tb.t_lin + (matte_bgra & 0xffu)), mg = __ldg(tb.t_lin + ((matte_bgra >> 8) & 0xffu)), mr = __ldg(tb.t_lin + ((matte_bgra >> 16) & 0xffu));
-    const uint32_t total = w * h;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const uint32_t total = w * h, step = gridDim.x * blockDim.x, first = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t n = first < total ? (total - 1u - first) / step + 1u : 0u;     // counted first, as in color_matrix_kernel
+    uint32_t i = first;
+    for (uint32_t k = 0; k < n; ++k, i += step) {
         const uint32_t y = i / w, x = i - y * w;
         uint32_t* p = reinterpret_cast<uint32_t*>(px + (size_t)y * stride) + x;
         const uint32_t v = *p;

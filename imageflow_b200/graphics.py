@@ -1568,11 +1568,12 @@ class Batch:
         self._keep.clear()
 
     def host_profile(self) -> dict:
-        """seconds the calling thread has spent inside enqueue calls so far, by part (ifb200_batch_host_profile)"""
-        v = (C.c_double * 8)()
-        lib().ifb200_batch_host_profile(self._h, v, 8)
+        """seconds the calling thread has spent inside enqueue calls so far, by part, and counts of what they did, among them the
+        row bands of the ring kernel's launches (ifb200_batch_host_profile)"""
+        v = (C.c_double * 9)()
+        lib().ifb200_batch_host_profile(self._h, v, 9)
         return {"enqueue_s": v[0], "plans_s": v[1], "staging_slots_s": v[2], "staging_memcpy_s": v[3], "table_uploads_s": v[4],
-                "table_uploads": int(v[5]), "staged_bytes": int(v[6]), "pinned_allocs": int(v[7])}
+                "table_uploads": int(v[5]), "staged_bytes": int(v[6]), "pinned_allocs": int(v[7]), "ring_bands": int(v[8])}
 
     @property
     def kernel_launches(self) -> int:

@@ -414,7 +414,8 @@ uint64_t ifb200_batch_kernel_launches(const ifb200_batch* b);   /* total kernels
 /* Where the calling thread has spent its enqueue calls so far, in seconds (inclusive: [1..4] are parts of [0]; [2] and [3] parts of [4]):
    out[0] whole enqueue calls, [1] building plans, [2] pinned staging slots (search + cudaMallocHost), [3] memcpy of tables into
    them, [4] table uploads (allocation + [2] + [3] + cudaMemcpyAsync + events); then counts: [5] table uploads, [6] bytes staged,
-   [7] cudaMallocHost calls.  Fills min(n, 8) entries, returns 8. */
+   [7] cudaMallocHost calls, [8] row bands of the ring kernel's launches (summed over launches).  Fills min(n, 9) entries,
+   returns 9. */
 int      ifb200_batch_host_profile(const ifb200_batch* b, double* out, int n);
 uint64_t ifb200_batch_fused_jobs(const ifb200_batch* b);        /* jobs that took the streaming ring kernel */
 uint64_t ifb200_batch_generic_jobs(const ifb200_batch* b);      /* jobs that took the generic pair */
