@@ -22,7 +22,8 @@ Host-side mirror of the reference seam (paths relative to the imageflow checkout
   flow/nodes/watermark.rs, imageflow_riapi ir4/layout.rs + sizing.rs  Watermark: its layout (watermark_layout, process_constraint) and
       every frame's composite from one resample per distinct watermark (Batch.watermark; RIAPI's placement as riapi_watermark_placement)
   graphics/swizzle.rs, bitmaps.rs:1284-1345  rgb_to_bgra, copy_swap_br, gray_to_bgra, gray_alpha_to_bgra, to_vec_rgb: decoder rows into
-      BGRA and encoder rows out of it, batched (Batch.pixel_convert over PixelRows; Batch.to_bgra / from_bgra for one tensor)
+      BGRA and encoder rows out of it, batched (Batch.pixel_convert over PixelRows; Batch.to_bgra / from_bgra for one tensor); an
+      RGB24 / RGBA32 conversion whose only consumer is the resample folded into its reads (Batch.scale_and_render_rows)
   c_components/lib/codecs_jpeg_idct_fast.c  flow_scale_spatial[_srgb]_NxN (decode-time JPEG block scalers)
 All arithmetic runs in hand-written sm_90a kernels inside libifb200.so (include/ifb200.h);
 this package only marshals arguments.  Nothing here imports the CPU oracle.
@@ -38,7 +39,7 @@ from .graphics import (Batch, apply_matte, BitmapCompositing, BitmapWindow, Erro
                        riapi_color_steps, Watermark, WatermarkConstraintBox, WatermarkConstraintMode, ConstraintGravity, WatermarkDraw,
                        process_constraint, watermark_layout, riapi_watermark_placement, PixelRows, RgbToBgra, RgbaToBgra, GrayToBgra,
                        GrayAlphaToBgra, BgraToRgb, pixel_op_for, CropWhitespace, riapi_trim_steps, crop_whitespace_bounds)
-from ._lib import LIB_PATH, ResampleDesc, lib
+from ._lib import LIB_PATH, ResampleDesc, RowsResampleDesc, lib
 
 __all__ = [
     "Batch", "apply_matte", "BitmapCompositing", "BitmapWindow", "ErrorKind", "Filter", "FlowError", "ScaleAndRenderParams",
@@ -51,5 +52,5 @@ __all__ = [
     "riapi_flip_steps", "apply_orientation", "oriented_source_window", "ColorMatrixSrgb", "ColorFilterSrgb", "WhiteBalanceHistogramAreaThresholdSrgb",
     "riapi_color_steps", "Watermark", "WatermarkConstraintBox", "WatermarkConstraintMode", "ConstraintGravity", "WatermarkDraw",
     "process_constraint", "watermark_layout", "riapi_watermark_placement", "PixelRows", "RgbToBgra", "RgbaToBgra", "GrayToBgra",
-    "GrayAlphaToBgra", "BgraToRgb", "pixel_op_for", "CropWhitespace", "riapi_trim_steps", "crop_whitespace_bounds", "LIB_PATH", "ResampleDesc", "lib",
+    "GrayAlphaToBgra", "BgraToRgb", "pixel_op_for", "CropWhitespace", "riapi_trim_steps", "crop_whitespace_bounds", "LIB_PATH", "ResampleDesc", "RowsResampleDesc", "lib",
 ]

@@ -22,7 +22,7 @@ SYMBOLS = [
     "ifb200_batch_fused_jobs", "ifb200_batch_generic_jobs", "ifb200_batch_tile_jobs", "ifb200_batch_ring_status", "ifb200_hv_plan_tables",
     "ifb200_block_scale_u8", "ifb200_batch_block_scale", "ifb200_round_corners_bgra8", "ifb200_batch_round_corners",
     "ifb200_batch_canvas", "ifb200_batch_orient", "ifb200_batch_color_chain", "ifb200_batch_watermark",
-    "ifb200_batch_pixel_convert", "ifb200_batch_enqueue_oriented", "ifb200_batch_detect_content_many",
+    "ifb200_batch_pixel_convert", "ifb200_batch_enqueue_oriented", "ifb200_batch_enqueue_rows", "ifb200_batch_detect_content_many",
 ]
 
 
@@ -41,6 +41,11 @@ class ResampleDesc(C.Structure):
 class OrientedResampleDesc(C.Structure):
     """struct ifb200_oriented_resample_desc"""
     _fields_ = [("draw", ResampleDesc), ("orientation", C.c_int32)]
+
+
+class RowsResampleDesc(C.Structure):
+    """struct ifb200_rows_resample_desc"""
+    _fields_ = [("draw", ResampleDesc), ("format", C.c_int32)]
 
 
 class RoundCornersDesc(C.Structure):
@@ -172,6 +177,8 @@ def lib() -> C.CDLL:
     L.ifb200_batch_enqueue.restype = C.c_int
     L.ifb200_batch_enqueue_oriented.argtypes = [C.c_void_p, C.POINTER(OrientedResampleDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_enqueue_oriented.restype = C.c_int
+    L.ifb200_batch_enqueue_rows.argtypes = [C.c_void_p, C.POINTER(RowsResampleDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
+    L.ifb200_batch_enqueue_rows.restype = C.c_int
     L.ifb200_batch_color_matrix.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, f32p, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_color_matrix.restype = C.c_int
     L.ifb200_batch_sync.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]

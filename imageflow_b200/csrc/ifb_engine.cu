@@ -412,11 +412,21 @@ int hv_cols(int av, int ch, int option);
 // ------------------------------------------------------------------------------------------------
 // ring kernel dispatch table
 using HvFn = void (*)(const JobDev*, const HvTmap*, Tables, HvPlanDev, uint32_t, uint32_t*);
-struct HvEntry { int av, ch; HvFn fn[3][3]; int threads, warps, max_cols, ng; uint32_t (*smem)(uint32_t); };   // fn[ORI][EPI]; EPI: general, simple + linear, simple + sRGB
+// fn[ORI][EPI] reads BGRA frames, rows[SRC - 1][EPI] the rows of ifb200_batch_enqueue_rows (HV_SRC_RGBA, HV_SRC_RGB24); EPI: general,
+// simple + linear, simple + sRGB
+struct HvEntry { int av, ch; HvFn fn[3][3]; int threads, warps, max_cols, ng; uint32_t (*smem)(uint32_t); HvFn rows[2][3]; };
 template <int AV, int CH> uint32_t hv_smem_bytes(uint32_t sb_low16) { return hv_total_bytes<AV, CH>(sb_low16); }
 #define IFB_HV_EPI(AV_, CH_, O_) {hv_ring_kernel<AV_, CH_, 0, O_>, hv_ring_kernel<AV_, CH_, 1, O_>, hv_ring_kernel<AV_, CH_, 2, O_>}
+// The RGB24 form with the general store epilogue at ring depth 6 and three channels spills (one register over the 128 of 16 warps):
+// it is not compiled, and its jobs take the generic pair (enqueue_locked)
+template <int AV, int CH> constexpr HvFn kRgb24General = hv_ring_kernel<AV, CH, 0, HV_ORI_NONE, HV_SRC_RGB24>;
+template <> constexpr HvFn kRgb24General<6, 3> = nullptr;
+#define IFB_HV_SRC(AV_, CH_) {{hv_ring_kernel<AV_, CH_, 0, HV_ORI_NONE, HV_SRC_RGBA>, hv_ring_kernel<AV_, CH_, 1, HV_ORI_NONE, HV_SRC_RGBA>, \
+                               hv_ring_kernel<AV_, CH_, 2, HV_ORI_NONE, HV_SRC_RGBA>}, \
+                              {kRgb24General<AV_, CH_>, hv_ring_kernel<AV_, CH_, 1, HV_ORI_NONE, HV_SRC_RGB24>, hv_ring_kernel<AV_, CH_, 2, HV_ORI_NONE, HV_SRC_RGB24>}}
 #define IFB_HV(AV_, CH_) {AV_, CH_, {IFB_HV_EPI(AV_, CH_, HV_ORI_NONE), IFB_HV_EPI(AV_, CH_, HV_ORI_FLIP), IFB_HV_EPI(AV_, CH_, HV_ORI_TRANSPOSE)}, \
-                          HvCfg<AV_, CH_>::kThreads, HvCfg<AV_, CH_>::kWarps, HvCfg<AV_, CH_>::kMaxCols, HvCfg<AV_, CH_>::kNG, hv_smem_bytes<AV_, CH_>}
+                          HvCfg<AV_, CH_>::kThreads, HvCfg<AV_, CH_>::kWarps, HvCfg<AV_, CH_>::kMaxCols, HvCfg<AV_, CH_>::kNG, hv_smem_bytes<AV_, CH_>, \
+                          IFB_HV_SRC(AV_, CH_)}
 const HvEntry kHv[] = {IFB_HV(4, 3), IFB_HV(4, 4), IFB_HV(6, 3), IFB_HV(6, 4)};
 const HvEntry* find_hv(int av, int ch) {
     for (const auto& e : kHv) if (e.av == av && e.ch == ch) return &e;
@@ -444,12 +454,15 @@ using TmapEncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 struct TmapKey {
     uintptr_t base; uint32_t w, h, stride; bool transposed;   // transposed: the box of the oriented ring kernel for flags 5..8
-    bool operator==(const TmapKey& o) const { return base == o.base && w == o.w && h == o.h && stride == o.stride && transposed == o.transposed; }
+    bool bytes;                                                // bytes: RGB24 rows, a UINT8 tensor w bytes wide (RGBA32 shares the u32 map)
+    bool operator==(const TmapKey& o) const {
+        return base == o.base && w == o.w && h == o.h && stride == o.stride && transposed == o.transposed && bytes == o.bytes;
+    }
 };
 struct TmapKeyHash {
     size_t operator()(const TmapKey& k) const {
         uint64_t x = (uint64_t)k.base * 0x9E3779B97F4A7C15ull;
-        x ^= ((uint64_t)k.w << 32 | k.h) * 0xC2B2AE3D27D4EB4Full; x ^= ((uint64_t)k.stride * 2 + k.transposed) * 0x165667B19E3779F9ull;
+        x ^= ((uint64_t)k.w << 32 | k.h) * 0xC2B2AE3D27D4EB4Full; x ^= ((uint64_t)k.stride * 4 + k.transposed * 2 + k.bytes) * 0x165667B19E3779F9ull;
         return (size_t)(x ^ (x >> 29));
     }
 };
@@ -746,20 +759,22 @@ void host_tables() {
 // TMA descriptor of one input bitmap for the ring kernel: u32 pixels, box 16 x 32, SWIZZLE_64B, out-of-bounds = 0; `transposed`
 // (the oriented kernel of flags 5..8): box 32 x 16, no swizzle.  d is the window as stored.
 // The base is aligned down to 16 bytes (a window may start at any pixel: bitmaps.rs:413-431); the kernel adds the 0..3 pixels
-// it was moved by to its x coordinates.
-const HvTmap& tmap_for(ifb200_batch* b, const ifb200_resample_desc& d, uint32_t* xoff_out, bool transposed = false) {
+// it was moved by to its x coordinates.  `bytes` (RGB24 rows of ifb200_batch_enqueue_rows): u8 elements, the 0..15 bytes between
+// the base and d.in plus 3 in_w bytes per row, box 64 x 32, SWIZZLE_64B; *xoff_out is then those 0..15 bytes.
+const HvTmap& tmap_for(ifb200_batch* b, const ifb200_resample_desc& d, uint32_t* xoff_out, bool transposed = false, bool bytes = false) {
     const uintptr_t addr = (uintptr_t)d.in;
     const uintptr_t base = addr & ~(uintptr_t)15;
-    const uint32_t xoff = (uint32_t)((addr - base) / 4);
+    const uint32_t xoff = bytes ? (uint32_t)(addr - base) : (uint32_t)((addr - base) / 4);
     *xoff_out = xoff;
-    const TmapKey key{base, d.in_w + xoff, d.in_h, d.in_stride, transposed};
+    const uint32_t w = bytes ? xoff + 3u * d.in_w : d.in_w + xoff;
+    const TmapKey key{base, w, d.in_h, d.in_stride, transposed, bytes};
     auto it = b->tmaps.find(key);
     if (it != b->tmaps.end()) return it->second;
     if (b->tmaps.size() > 65536) b->tmaps.clear();
     CUtensorMap tm;
-    const cuuint64_t dims[2] = {(cuuint64_t)d.in_w + xoff, (cuuint64_t)d.in_h};
+    const cuuint64_t dims[2] = {(cuuint64_t)w, (cuuint64_t)d.in_h};
     const cuuint64_t strides[1] = {(cuuint64_t)d.in_stride};
-    const cuuint32_t box[2] = {transposed ? 32u : 16u, transposed ? 16u : 32u};
+    const cuuint32_t box[2] = {bytes ? 64u : transposed ? 32u : 16u, transposed ? 16u : 32u};
     const cuuint32_t estr[2] = {1u, 1u};
     // L2 promotion: how much of a line a 64-byte box row pulls into L2 (IFB200_DEBUG_L2_PROMOTION = 0 / 64 / 128 / 256 for experiments)
     static const CUtensorMapL2promotion promo = [] {
@@ -767,7 +782,7 @@ const HvTmap& tmap_for(ifb200_batch* b, const ifb200_resample_desc& d, uint32_t*
         const int v = e ? atoi(e) : 256;
         return v == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : v == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : v == 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
     }();
-    const CUresult r = b->tmap_encode(&tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    const CUresult r = b->tmap_encode(&tm, bytes ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                       transposed ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_64B, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) IFB_THROW(IFB200_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) for a %ux%u bitmap, pitch %u", (int)r, d.in_w, d.in_h, d.in_stride);
     HvTmap h;
@@ -794,18 +809,21 @@ uint32_t ori_flips(int flag) {
 // ori[i] in 2..8: in_w x in_h is the ORIENTED size (swapped against the stored window for 5..8), the descriptors have been checked
 // as stored, and the plans are those of the oriented geometry.  Oriented jobs take the ring kernel's oriented forms or the generic
 // pair with the oriented H pass (there is no oriented tile kernel).
-void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n, cudaStream_t st, const int32_t* ori = nullptr) {
+// src != nullptr (enqueue_rows_locked): descs[i].in holds rows of format src[i] (HV_SRC_RGBA / HV_SRC_RGB24), checked by the
+// caller; these jobs take the ring kernel's row forms or the generic pair with hpass_rows_kernel (there is no tile-kernel form).
+void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n, cudaStream_t st, const int32_t* ori = nullptr,
+                    const int32_t* src = nullptr) {
     if (!descs && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
     if (n == 0) return;
     Tick tk_all(b->prof.enqueue);
     host_tables();
     DeviceScope dev_scope_(b->device);
-    if (!ori)
+    if (!ori && !src)
         for (size_t i = 0; i < n; ++i) validate(descs[i]);
     { Tick tk(b->prof.plans); b->prebuild_plans(descs, n); }
     // group jobs by (plan, kernel class)
     // kind: 0 generic pair, 1 ring kernel, 3 tile kernel (`variant` = its compile-time case)
-    struct Group { Plan* plan; int ch; int kind; bool simple; int variant; int ori; std::vector<size_t> idx; int cols_key = 0; };
+    struct Group { Plan* plan; int ch; int kind; bool simple; int variant; int ori; int src; std::vector<size_t> idx; int cols_key = 0; };
     std::vector<Group> groups;
     for (size_t i = 0; i < n; ++i) {
         Plan* pp; { Tick tk(b->prof.plans); pp = &b->plan_for(descs[i]); }
@@ -821,17 +839,26 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
         // the ring kernel's TMA box origins stay 16-byte aligned: with source x reversed, boxes start at W - 16 - x (flags 2, 3) or
         // W - 32 - y (flags 7, 8), so the stored width W (in_w, or in_h of the oriented plan for 5..8) must be a multiple of four
         if (oc != HV_ORI_NONE && (ori_flips(ori[i]) & JF_FLIP_X) && ((oc == HV_ORI_TRANSPOSE ? p.in_h : p.in_w) & 3u)) ring = false;
+        // rows: up-scales and 1:1 take the generic pair; RGB24 rows may start at any byte (the box origins are aligned below the
+        // window's first byte), so only the pitch must be a multiple of 16 bytes
+        const int sf = src ? src[i] : HV_SRC_BGRA;
+        if (sf != HV_SRC_BGRA) {
+            if (sf == HV_SRC_RGB24) ring = p.hv_ok && b->ring_ok && !b->force_generic && (d.in_stride % 16 == 0);
+            if (upscale) ring = false;
+        }
+        const bool simple = d.compose == IFB200_REPLACE_SELF && !d.color_matrix;   // store epilogue without composite / matrix code
+        if (ring && sf != HV_SRC_BGRA && !find_hv(p.av, ch)->rows[sf - 1][simple ? 1 : 0]) ring = false;   // a form not compiled
         if (ring && !(p.tile_ok && upscale) && !hv_host_ready(p, hv_cols(p.av, ch, b->strip_cols))) ring = false;   // windows wider than the weight table
         // the ring kernel streams every source row once and wins whenever rows outnumber outputs (down-scales);
         // for up-scales / 1:1 the tile kernel does less work per source pixel
-        const bool prefer_tile = oc == HV_ORI_NONE && p.tile_ok && !b->force_generic && (!ring || upscale);
+        const bool prefer_tile = oc == HV_ORI_NONE && sf == HV_SRC_BGRA && p.tile_ok && !b->force_generic && (!ring || upscale);
         const int kind = prefer_tile ? 3 : (ring ? 1 : 0);
-        const bool simple = d.compose == IFB200_REPLACE_SELF && !d.color_matrix;   // store epilogue without composite / matrix code
         // the ring kernel keeps ONE transfer table per CTA: jobs of different working spaces go to different launches
         const int variant = kind == 3 ? ((d.linear ? 1 : 0) | ((ch == 4 ? d.compose : 0) << 1) | (d.color_matrix ? 8 : 0)) : kind == 1 ? (d.linear ? 1 : 0) : 0;
         Group* g = nullptr;
-        for (auto& gg : groups) if (gg.plan == &p && gg.ch == ch && gg.kind == kind && gg.simple == simple && gg.variant == variant && gg.ori == oc) { g = &gg; break; }
-        if (!g) { groups.push_back(Group{&p, ch, kind, simple, variant, oc, {}}); g = &groups.back(); }
+        for (auto& gg : groups)
+            if (gg.plan == &p && gg.ch == ch && gg.kind == kind && gg.simple == simple && gg.variant == variant && gg.ori == oc && gg.src == sf) { g = &gg; break; }
+        if (!g) { groups.push_back(Group{&p, ch, kind, simple, variant, oc, sf, {}}); g = &groups.back(); }
         g->idx.push_back(i);
     }
     // Strip width of every ring group: the widest (least halo) that still gives every warp of the device an item; a launch for one
@@ -910,7 +937,7 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
             if (ht) {
                 ifb200_resample_desc stored = descs[i];                   // the TMA descriptor describes the window as stored
                 if (g.ori == HV_ORI_TRANSPOSE) std::swap(stored.in_w, stored.in_h);
-                uint32_t xoff = 0; ht[pos] = tmap_for(b, stored, &xoff, g.ori == HV_ORI_TRANSPOSE); hj[pos].in_xoff = xoff;
+                uint32_t xoff = 0; ht[pos] = tmap_for(b, stored, &xoff, g.ori == HV_ORI_TRANSPOSE, g.src == HV_SRC_RGB24); hj[pos].in_xoff = xoff;
             }
             ++pos;
         }
@@ -986,7 +1013,8 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
             pl.hw = ht.blob.at<float>(ht.o_hw); pl.hdone = ht.blob.at<uint8_t>(ht.o_hdone);
             pl.vw = ht.blob.at<float>(ht.o_vw); pl.vdone = ht.blob.at<uint8_t>(ht.o_vdone);
             pl.hw_stride = ht.hw_stride;
-            HvFn fn = he->fn[g.ori][g.simple ? ((g.variant & 1) ? 1 : 2) : 0];        // the ring kernel's launches are per working space (variant bit 0 = linear)
+            const int epi = g.simple ? ((g.variant & 1) ? 1 : 2) : 0;       // the ring kernel's launches are per working space (variant bit 0 = linear)
+            HvFn fn = g.src != HV_SRC_BGRA ? he->rows[g.src - 1][epi] : he->fn[g.ori][epi];
             const size_t smem = he->smem(b->smem_base_low16);
             if (!b->hv_attr_set.count((const void*)fn)) {
                 CUDA_OK(cudaFuncSetAttribute((const void*)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1008,7 +1036,11 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
             AsyncFree inter_guard{inter, st};
             for (size_t off = 0; off < nj; off += chunk) {
                 const size_t cnt = std::min(chunk, nj - off);
-                if (g.ori == HV_ORI_NONE) {
+                if (g.src != HV_SRC_BGRA) {
+                    dim3 gh((p.out_w + 127) / 128, std::min<uint32_t>(p.in_h, 65535u), (unsigned)cnt);
+                    if (g.src == HV_SRC_RGB24) hpass_rows_kernel<3><<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_h, p.out_w, inter);
+                    else hpass_rows_kernel<4><<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_h, p.out_w, inter);
+                } else if (g.ori == HV_ORI_NONE) {
                     dim3 gh((p.out_w + 127) / 128, std::min<uint32_t>(p.in_h, 65535u), (unsigned)cnt);
                     hpass_generic_kernel<<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_h, p.out_w, inter);
                 } else if (g.ori == HV_ORI_FLIP) {
@@ -1058,6 +1090,46 @@ void enqueue_oriented_locked(ifb200_batch* b, const ifb200_oriented_resample_des
     }
     enqueue_locked(b, plain.data(), plain.size(), st);
     enqueue_locked(b, turned.data(), turned.size(), st, flags.data());
+}
+
+// ifb200_batch_enqueue_rows: every descriptor is checked -- its format, the resample's own rules (resample_check, with the rows'
+// rules in place of a BGRA row's), then the rows' -- and every plan built before anything is enqueued; then all jobs go through
+// enqueue_locked's row forms.
+void enqueue_rows_locked(ifb200_batch* b, const ifb200_rows_resample_desc* d, size_t n, cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    if (n == 0) return;
+    std::vector<ifb200_resample_desc> draws(n);
+    std::vector<int32_t> src(n);
+    for (size_t i = 0; i < n; ++i) {
+        const ifb200_resample_desc& r = d[i].draw;
+        const int32_t f = d[i].format;
+        if (f == IFB200_PIXEL_GRAY_TO_BGRA || f == IFB200_PIXEL_GRAY_ALPHA_TO_BGRA)
+            IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "rows resample job %zu: format %d (%s) has no resample form; convert the rows with "
+                      "ifb200_batch_pixel_convert, then resample the BGRA frame with ifb200_batch_enqueue", i, (int)f,
+                      f == IFB200_PIXEL_GRAY_TO_BGRA ? "Gray8" : "GrayAlpha8");
+        if (f != IFB200_PIXEL_RGB24_TO_BGRA && f != IFB200_PIXEL_RGBA_TO_BGRA)
+            IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "rows resample job %zu: format %d is not IFB200_PIXEL_RGB24_TO_BGRA (0) or "
+                      "IFB200_PIXEL_RGBA_TO_BGRA (1)", i, (int)f);
+        ifb200_resample_desc c = r;                                       // every rule but the row's
+        c.in_w = r.in_w ? 1u : 0u; c.in_stride = 4u;
+        int code = 0;
+        const std::string why = ifb::resample_check(c, &code);
+        if (!why.empty()) IFB_THROW(code, "rows resample job %zu: %s", i, why.c_str());
+        const uint32_t bpp = f == IFB200_PIXEL_RGB24_TO_BGRA ? 3u : 4u;
+        if (r.in_stride < (uint64_t)r.in_w * bpp)
+            IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "rows resample job %zu: stride %u smaller than a row of %u %s pixels", i, r.in_stride,
+                      r.in_w, bpp == 3u ? "RGB24" : "RGBA32");
+        if (bpp == 4u && (((uintptr_t)r.in & 3) || (r.in_stride & 3)))
+            IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "rows resample job %zu: RGBA32 rows need a 4-byte aligned pointer and stride", i);
+        draws[i] = r;
+        src[i] = bpp == 3u ? HV_SRC_RGB24 : HV_SRC_RGBA;
+    }
+    {
+        Tick tk(b->prof.plans);
+        b->prebuild_plans(draws.data(), n);
+        for (const auto& r : draws) b->plan_for(r);                      // may throw: nothing enqueued yet
+    }
+    enqueue_locked(b, draws.data(), n, st, nullptr, src.data());
 }
 
 // The argument checks of a BGRA window, shared by the device and the host-buffer form of each operation: a null pointer, or a stride
@@ -1860,6 +1932,10 @@ int ifb200_batch_enqueue(ifb200_batch* b, const ifb200_resample_desc* descs, siz
 
 int ifb200_batch_enqueue_oriented(ifb200_batch* b, const ifb200_oriented_resample_desc* d, size_t n, void* stream, char* err, size_t cap) {
     return with_batch(b, stream, err, cap, [&](cudaStream_t st) { enqueue_oriented_locked(b, d, n, st); });
+}
+
+int ifb200_batch_enqueue_rows(ifb200_batch* b, const ifb200_rows_resample_desc* d, size_t n, void* stream, char* err, size_t cap) {
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { enqueue_rows_locked(b, d, n, st); });
 }
 
 int ifb200_batch_color_matrix(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, const float m[25],

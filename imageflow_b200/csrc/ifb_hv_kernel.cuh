@@ -59,6 +59,10 @@ struct alignas(64) HvTmap { unsigned char bytes[128]; };              // CUtenso
 // either axis walked backwards (1); flags 5..8, the transposed box, the lanes along source columns (2).  Which axes run backwards is
 // per job (JF_FLIP_X / JF_FLIP_Y).
 enum : int { HV_ORI_NONE = 0, HV_ORI_FLIP = 1, HV_ORI_TRANSPOSE = 2 };
+// The source pixel format an instantiation reads (template parameter SRC, ifb200_batch_enqueue_rows): BGRA32 (0); RGBA32 (1), the
+// same u32 box, the table look-ups taking blue from byte 2 and red from byte 0; RGB24 (2), a UINT8 tensor read in boxes of 64 bytes
+// x 32 rows, 16 pixels (48 bytes) at a constant offset r inside each box.  Only the stored frame (ORI = HV_ORI_NONE) has these forms.
+enum : int { HV_SRC_BGRA = 0, HV_SRC_RGBA = 1, HV_SRC_RGB24 = 2 };
 
 #ifndef IFB_HV_MAXCOLS4
 #define IFB_HV_MAXCOLS4 64             // widest strip of the ring-depth-4 variants (V accumulators: 12 or 16 registers per 16 columns)
@@ -319,10 +323,18 @@ __device__ __forceinline__ uint32_t hv_finish_pixel(float b, float g, float r, f
 // of four box rows per chunk, four conflict-free 4-byte loads.  Boxes that reach past the bitmap (negative coordinates included)
 // are zero-filled by the TMA unit; their samples carry zero weights.  Box origins along source x stay multiples of four pixels (16
 // bytes), as for the stored frame: see the band start below and the engine's choice of jobs for the ring kernel.
-template <int AV, int CH, int EPI, int ORI = HV_ORI_NONE>
+// SRC != HV_SRC_BGRA: the resample of to_bgra(rows) (ifb200_batch_enqueue_rows); the plan, the V pass and the store are those of the
+// BGRA frame.  RGBA32 reads the BGRA box and swaps blue and red in the look-ups' byte selectors.  RGB24: the tensor is the rows'
+// bytes from the 16-byte aligned address at or below `in` (in_xoff = the 0..15 bytes between them, the "phase"), phase + 3 in_w
+// bytes wide, zero-filled beyond; the 16 pixels of a box start at byte phase + 3x, so the box origin (phase + 3x) & ~15 stays
+// 16-byte aligned and the pixels sit at byte r = (phase + 3x) & 15 of every box row, the same r all along the stream (48 = 0 mod
+// 16; r + 48 <= 63).  A lane's chunk k is bytes r + 12k .. r + 12k + 11 of its row: four 4-byte loads (words r/4 + 3k ..) and byte
+// permutes give its four pixels as words with red in byte 0, green in byte 1, blue in byte 2 (byte 3 unused: alpha is 255).
+template <int AV, int CH, int EPI, int ORI = HV_ORI_NONE, int SRC = HV_SRC_BGRA>
 __global__ void __launch_bounds__(HvCfg<AV, CH>::kThreads, 1)
 hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps, Tables tb, HvPlanDev pl, uint32_t n_jobs,
                uint32_t* __restrict__ counters) {
+    static_assert(SRC == HV_SRC_BGRA || ORI == HV_ORI_NONE, "row formats are read without orientation");
     using C = HvCfg<AV, CH>;
     constexpr int AVP = C::kAvp, NG = C::kNG, NP = C::kNP, S = C::kStages, CG = C::kCG;
     constexpr uint32_t kRec = (uint32_t)AVP * 4u;                          // bytes per H weight record (one source column)
@@ -417,17 +429,22 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
             const int bY0 = (int)uni((uint32_t)bd_.Y0), bY1 = (int)uni((uint32_t)bd_.Y1);
             const uint32_t flags = uni(job.flags);
             const int nrb = (bNr + 31) >> 5;
-            const int x_origin = sK0 + (int)uni(job.in_xoff);
+            // where the stream starts in the tensor: pixel sK0 + xoff; RGB24, byte phase + 3 sK0 (its boxes at x & ~15, its pixels at
+            // r = x_origin & 15 of every box row: no register beyond the BGRA form's, which is at the register budget)
+            constexpr int kBoxX = SRC == HV_SRC_RGB24 ? 48 : 16;               // tensor elements per 16 pixels
+            const int x_origin = SRC == HV_SRC_RGB24 ? (int)uni(job.in_xoff) + 3 * sK0 : sK0 + (int)uni(job.in_xoff);
 
             // ---- TMA pipeline state: boxes are fetched row block by row block, left to right
-            const int x_end = x_origin + nst * 16;
+            const int x_end = x_origin + nst * kBoxX;
             int tma_x = x_origin, tma_y = bJ0, tma_left = nrb * nst, is_s = 0;   // next box to fetch, boxes not fetched yet, the ring slot it goes to
             auto issue = [&](const uint32_t zero_dep) {                    // zero_dep: 0, computed from what the slot's last load returned
                 hv::warp_sync();                                           // every lane has read what the refilled slot held
                 if (leader) {
                     const uint32_t bar = mb + 8u * (uint32_t)is_s;
                     hv::mbar_expect_tx(bar, (uint32_t)C::kStageBytes);
-                    if constexpr (ORI == HV_ORI_NONE) {
+                    if constexpr (ORI == HV_ORI_NONE && SRC == HV_SRC_RGB24) {   // 48 bytes per 16 pixels: origins stay 16-byte aligned
+                        hv::tma_load_box(stb + (uint32_t)is_s * C::kStageBytes, tm, (tma_x & ~15) + (int)zero_dep, tma_y, bar);
+                    } else if constexpr (ORI == HV_ORI_NONE) {
                         hv::tma_load_box(stb + (uint32_t)is_s * C::kStageBytes, tm, tma_x + (int)zero_dep, tma_y, bar);
                     } else {
                         // the box of oriented columns [tma_x, +16) x rows [tma_y, +32) in the stored frame (pl.in_w x pl.in_h is the
@@ -440,7 +457,7 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
                     }
                 }
                 --tma_left; is_s ^= 1;
-                tma_x += 16;
+                tma_x += kBoxX;
                 if (tma_x == x_end) { tma_x = x_origin; tma_y += 32; }
             };
             static_assert(S == 2, "the slot bookkeeping below toggles between two slots");
@@ -457,7 +474,16 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
                                                    : (lrow * 4u) | (rev_s ? 15u << 7 : 0u);
             // chunk k (four oriented columns) of this lane's row in the stage at sb_ (the stage, + lane * 64 for the stored frame)
             auto chunk = [&](const uint32_t sb_, const uint32_t k_) -> uint4 {
-                if constexpr (ORI == HV_ORI_NONE) {
+                if constexpr (ORI == HV_ORI_NONE && SRC == HV_SRC_RGB24) {
+                    // words q .. q + 3 (q = r/4 + 3k; q + 3 <= 15) at their swizzled places in the row, then bytes r + 12k .. r + 12k + 11
+                    // as y0 y1 y2 = (r0 g0 b0 r1) (g1 b1 r2 g2) (b2 r3 g3 b3) (a byte permute that shifts by r & 3 bytes), then one word
+                    // per pixel
+                    const uint32_t a = ((uint32_t)x_origin & 12u) + 12u * k_, fsel = 0x3210u + 0x1111u * ((uint32_t)x_origin & 3u);
+                    const uint32_t x0 = hv::lds_u32(sb_ + (a ^ swz)), x1 = hv::lds_u32(sb_ + ((a + 4u) ^ swz));
+                    const uint32_t x2 = hv::lds_u32(sb_ + ((a + 8u) ^ swz)), x3 = hv::lds_u32(sb_ + ((a + 12u) ^ swz));
+                    const uint32_t y0 = hv::prmt(x0, x1, fsel), y1 = hv::prmt(x1, x2, fsel), y2 = hv::prmt(x2, x3, fsel);
+                    return make_uint4(y0, hv::prmt(y0, y1, 0x6543u), hv::prmt(y1, y2, 0x5432u), y2 >> 8);
+                } else if constexpr (ORI == HV_ORI_NONE) {
                     return hv::lds_u32x4(sb_ + ((k_ << 4) ^ swz));
                 } else if constexpr (ORI == HV_ORI_FLIP) {
                     const uint4 v = hv::lds_u32x4(sb_ + ((k_ << 4) ^ lo));
@@ -512,10 +538,12 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
                 // converted (its table look-ups are in flight) and its weight record fetched.
                 float P0[CH], P1[CH];
                 float2 W0[NP], W1[NP];
+                // the bytes of blue and red in a pixel word: 0 and 2 for BGRA, 2 and 0 for the row formats (RGB24 has no alpha byte: 255)
+                constexpr uint32_t kBB = SRC == HV_SRC_BGRA ? 0u : 2u, kBR = 2u - kBB;
                 auto conv = [&](float (&P)[CH], const uint32_t v) {
-                    P[0] = hv::lut_gather<0x6504>(v, lane4); P[1] = hv::lut_gather<0x6514>(v, lane4); P[2] = hv::lut_gather<0x6524>(v, lane4);
+                    P[0] = hv::lut_gather<0x6504u | (kBB << 4)>(v, lane4); P[1] = hv::lut_gather<0x6514>(v, lane4); P[2] = hv::lut_gather<0x6504u | (kBR << 4)>(v, lane4);
                     if (CH == 4) {                                         // alpha table entry == a * (1/255f) (color.rs:38): computed, not gathered
-                        const float af = __fmul_rn(__uint2float_rn(v >> 24), 1.0f / 255.0f);
+                        const float af = __fmul_rn(__uint2float_rn(SRC == HV_SRC_RGB24 ? 255u : v >> 24), 1.0f / 255.0f);
                         P[0] = __fmul_rn(P[0], af); P[1] = __fmul_rn(P[1], af); P[2] = __fmul_rn(P[2], af); P[CH - 1] = af;
                     }
                 };
@@ -567,8 +595,8 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
                     rawB = chunk(sbase, ((pc & 1u) << 1) | 1u);
                     if ((pc & 1u) && more) {
                         cs_s ^= 1;
-                        // (transposed: the chunk is four loads, and the refill waits for all of them)
-                        if (tma_left > 0) issue(hv::zero_after(ORI == HV_ORI_TRANSPOSE ? rawB.x ^ rawB.y ^ rawB.z ^ rawB.w : rawB.x, pl.zero));
+                        // (transposed and RGB24: the chunk is four loads, and the refill waits for all of them; RGB24's .x and .w depend on all four)
+                        if (tma_left > 0) issue(hv::zero_after(ORI == HV_ORI_TRANSPOSE ? rawB.x ^ rawB.y ^ rawB.z ^ rawB.w : SRC == HV_SRC_RGB24 ? rawB.x ^ rawB.w : rawB.x, pl.zero));
                         hv::mbar_wait(mb + 8u * (uint32_t)cs_s, (par >> cs_s) & 1u);
                         par ^= 1u << cs_s;
                         sbase = stb + (uint32_t)cs_s * C::kStageBytes + (ORI == HV_ORI_NONE ? (uint32_t)lane * 64u : 0u);

@@ -104,6 +104,43 @@ __global__ void __launch_bounds__(128) hpass_oriented_kernel(const JobDev* __res
     }
 }
 
+// The H pass of the rows resample (ifb200_batch_enqueue_rows): hpass_generic_kernel's chain, in the same order, over the taps of
+// output column X, each tap read from decoder rows of BPP bytes per pixel and converted as ifb200_pixel_convert_desc converts it
+// (opaque = 0) -- RGBA32 (BPP 4): (r, g, b, a) -> (b, g, r, a), one aligned 4-byte load; RGB24 (BPP 3): (r, g, b) -> (b, g, r, 255),
+// three byte loads at any address.  Writes the intermediate vpass_generic_kernel reads.
+template <int BPP>
+__global__ void __launch_bounds__(128) hpass_rows_kernel(const JobDev* __restrict__ jobs, Tables tb, AxisDev ah,
+                                                         uint32_t in_h, uint32_t out_w, float4* __restrict__ inter) {
+    const uint32_t X = blockIdx.x * blockDim.x + threadIdx.x;
+    const JobDev& job = jobs[blockIdx.z];
+    if (X >= out_w) return;
+    const bool am = job.flags & JF_ALPHA;
+    const float* __restrict__ T = (job.flags & JF_LINEAR) ? tb.t_lin : tb.t_srgb;
+    const uint32_t l = ah.left[X], r = ah.right[X];
+    const float* __restrict__ w = ah.w + ah.off[X];
+    for (uint32_t j = blockIdx.y; j < in_h; j += gridDim.y) {
+        const uint8_t* __restrict__ src = job.in + (size_t)j * job.in_stride;
+        float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+        for (uint32_t k = l; k <= r; ++k) {
+            uint32_t px;                                               // the tap as a BGRA word
+            if constexpr (BPP == 3) {
+                const uint8_t* p = src + (size_t)k * 3;
+                px = (uint32_t)__ldg(p + 2) | ((uint32_t)__ldg(p + 1) << 8) | ((uint32_t)__ldg(p) << 16) | 0xff000000u;
+            } else {
+                px = __byte_perm(__ldg(reinterpret_cast<const uint32_t*>(src) + k), 0u, 0x3012);
+            }
+            const float wt = __ldg(w + (k - l));
+            float pb = __ldg(T + (px & 0xffu)), pg = __ldg(T + ((px >> 8) & 0xffu)), pr = __ldg(T + ((px >> 16) & 0xffu)), pa = 0.0f;
+            if (am) {
+                pa = __ldg(tb.t_srgb + (px >> 24));
+                pb = __fmul_rn(pb, pa); pg = __fmul_rn(pg, pa); pr = __fmul_rn(pr, pa);
+            }
+            a0 = __fmaf_rn(wt, pb, a0); a1 = __fmaf_rn(wt, pg, a1); a2 = __fmaf_rn(wt, pr, a2); a3 = __fmaf_rn(wt, pa, a3);
+        }
+        inter[((size_t)blockIdx.z * in_h + j) * out_w + X] = make_float4(a0, a1, a2, a3);
+    }
+}
+
 __global__ void __launch_bounds__(128) vpass_generic_kernel(const JobDev* __restrict__ jobs, Tables tb, AxisDev av,
                                                             uint32_t in_h, uint32_t out_w, uint32_t out_h,
                                                             const float4* __restrict__ inter) {

@@ -10,7 +10,7 @@ from typing import Optional, Sequence
 import numpy as np
 
 from ._lib import (CanvasDesc, ColorDesc, ColorStep, DetectContentDesc, OrientDesc, OrientedResampleDesc, PixelConvertDesc, ResampleDesc, RoundCornersDesc,
-                   WatermarkDesc, lib)
+                   RowsResampleDesc, WatermarkDesc, lib)
 
 
 class Filter(enum.IntEnum):
@@ -1225,6 +1225,43 @@ class Batch:
         is rejected."""
         descs, keep = self.make_oriented_descs(jobs)
         self.enqueue_oriented(descs, stream, keep)
+
+    # channels of decoder rows -> their ifb200_pixel_op into BGRA (Gray8 and GrayAlpha8 are refused by ifb200_batch_enqueue_rows)
+    _ROWS_FORMAT = {3: 0, 4: 1, 1: 2, 2: 3}
+
+    def make_rows_descs(self, jobs):
+        """jobs: iterable of (rows, canvas BitmapWindow, ScaleAndRenderParams[, color_matrix[, alpha_meaningful]]); `rows` is anything
+        PixelRows.of() takes except a BitmapWindow (already BGRA: scale_and_render_many), its format given by its channels (3: RGB24,
+        4: RGBA32); alpha_meaningful defaults to what a decoder sets (False for RGB24, True for RGBA32)."""
+        jobs = list(jobs)
+        arr = (RowsResampleDesc * len(jobs))()
+        keep = []
+        for i, j in enumerate(jobs):
+            if isinstance(j[0], BitmapWindow):
+                raise FlowError(ErrorKind.InvalidArgument, f"rows resample job {i}: a BitmapWindow is already BGRA; resample it with "
+                                                           "scale_and_render_many")
+            rows = PixelRows.of(j[0])
+            am = (rows.channels == 4) if len(j) < 5 or j[4] is None else bool(j[4])
+            src = BitmapWindow(rows.ptr, rows.w, rows.h, rows.stride, alpha_meaningful=am, _keep=rows._keep)
+            _fill_desc(arr[i].draw, src, j[1], j[2], j[3] if len(j) > 3 else None, keep)
+            arr[i].format = self._ROWS_FORMAT.get(rows.channels, -1)
+            keep.append(rows._keep)
+        keep.append([j[1]._keep for j in jobs])                         # the bitmaps stay alive until sync() / close()
+        return arr, keep
+
+    def enqueue_rows(self, descs, stream=None, keep=None) -> None:
+        if keep:
+            self._keep.append(keep)
+        buf = C.create_string_buffer(512)
+        _check(lib().ifb200_batch_enqueue_rows(self._h, descs, len(descs), self._stream(stream), buf, 512), buf)
+
+    def scale_and_render_rows(self, jobs, stream=None) -> None:
+        """scale_and_render(to_bgra(rows), canvas, params) on DEVICE decoder rows without the BGRA frame being written: jobs: iterable
+        of (rows, canvas, ScaleAndRenderParams[, color_matrix[, alpha_meaningful]]) as make_rows_descs takes them -- e.g. nvJPEG's
+        (H, W, 3) RGB tensor or a PNG decoder's (H, W, 4) RGBA tensor.  to_bgra is the conversion of Batch.pixel_convert (RgbToBgra /
+        RgbaToBgra, not opaque).  Asynchronous on `stream`; nothing is written when an argument is rejected."""
+        descs, keep = self.make_rows_descs(jobs)
+        self.enqueue_rows(descs, stream, keep)
 
     def color_matrix(self, dev_ptr: int, w: int, h: int, stride: int, m, stream=None) -> None:
         mm = np.ascontiguousarray(m, np.float32).reshape(25)

@@ -293,6 +293,19 @@ typedef struct ifb200_pixel_convert_desc {
     int32_t        opaque;                  /* != 0: alpha = 255 in a 4-byte output */
 } ifb200_pixel_convert_desc;
 
+/* One resample of decoder rows: scale_and_render(to_bgra(draw.in, format), canvas, params), byte for byte, without the BGRA frame
+ * ever being written -- the decode -> DrawImageExact chain of a frame a GPU decoder wrote as interleaved rows (nvJPEG's RGB24, the
+ * PNG and WebP decoders' RGBA32).  to_bgra is the ifb200_pixel_convert_desc op `format` with opaque = 0.
+ *   draw    draw.in / in_w / in_h / in_stride: the rows as the decoder wrote them, in_w x in_h pixels; every other field as in
+ *           ifb200_batch_enqueue (draw.alpha_meaningful as the caller passes it: RGB24 with alpha_meaningful = 1 resamples an alpha of 255).
+ *   format  IFB200_PIXEL_RGB24_TO_BGRA (rows at any byte address, in_stride >= 3 in_w) or IFB200_PIXEL_RGBA_TO_BGRA (4-byte aligned
+ *           rows and stride, in_stride >= 4 in_w).  Gray8 and GrayAlpha8 rows are refused: convert them with
+ *           ifb200_batch_pixel_convert, then call ifb200_batch_enqueue. */
+typedef struct ifb200_rows_resample_desc {
+    ifb200_resample_desc draw;
+    int32_t format;
+} ifb200_rows_resample_desc;
+
 /* One frame of ifb200_batch_detect_content_many: detect_content (graphics/whitespace.rs:284-331) of the DEVICE BGRA window px
  * (w x h, row pitch `stride` bytes), grayscale Bgra32 when alpha_meaningful != 0 else Bgr32, edges where the Scharr value exceeds
  * `threshold`.  The limits are those of ifb200_batch_detect_content: a non-empty window, w and h below 2^31, threshold below 2^31. */
@@ -323,6 +336,14 @@ int  ifb200_batch_enqueue(ifb200_batch* b, const ifb200_resample_desc* descs, si
  * is enqueued, so an error means nothing is written.  ifb200_batch_fused_jobs / ifb200_batch_generic_jobs count these jobs too. */
 int  ifb200_batch_enqueue_oriented(ifb200_batch* b, const ifb200_oriented_resample_desc* d, size_t n, void* cuda_stream,
                                    char* err, size_t err_cap);
+/* n resamples of DEVICE decoder rows (ifb200_rows_resample_desc), asynchronous on `cuda_stream`, as ifb200_batch_enqueue.  The BGRA
+ * frame is never written: the conversion happens in the resample's source reads.  Down-scales run the streaming ring kernel (RGBA32:
+ * a 16-byte aligned window and pitch, as for BGRA; RGB24: a pitch that is a multiple of 16 bytes, the window at any byte);
+ * up-scales, 1:1, other windows and IFB200_OPT_FORCE_GENERIC run the generic pair with an H pass that converts its taps.  Every
+ * descriptor is checked ("rows resample job i: ...") and every plan built before anything is enqueued, so an error means nothing is
+ * written.  ifb200_batch_fused_jobs / ifb200_batch_generic_jobs count these jobs too. */
+int  ifb200_batch_enqueue_rows(ifb200_batch* b, const ifb200_rows_resample_desc* d, size_t n, void* cuda_stream,
+                               char* err, size_t err_cap);
 int  ifb200_batch_color_matrix(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride,
                                const float m[25], void* cuda_stream, char* err, size_t err_cap);
 int  ifb200_batch_apply_matte(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride,
