@@ -23,7 +23,8 @@ Host-side mirror of the reference seam (paths relative to the imageflow checkout
       every frame's composite from one resample per distinct watermark (Batch.watermark; RIAPI's placement as riapi_watermark_placement)
   graphics/swizzle.rs, bitmaps.rs:1284-1345  rgb_to_bgra, copy_swap_br, gray_to_bgra, gray_alpha_to_bgra, to_vec_rgb: decoder rows into
       BGRA and encoder rows out of it, batched (Batch.pixel_convert over PixelRows; Batch.to_bgra / from_bgra for one tensor); an
-      RGB24 / RGBA32 conversion whose only consumer is the resample folded into its reads (Batch.scale_and_render_rows)
+      RGB24 / RGBA32 conversion whose only consumer is the resample folded into its reads (Batch.scale_and_render_rows), also
+      together with an ApplyOrientation (Batch.scale_and_render_rows_oriented; a crop in between via oriented_source_rect)
   c_components/lib/codecs_jpeg_idct_fast.c  flow_scale_spatial[_srgb]_NxN (decode-time JPEG block scalers)
 All arithmetic runs in hand-written sm_90a kernels inside libifb200.so (include/ifb200.h);
 this package only marshals arguments.  Nothing here imports the CPU oracle.
@@ -35,11 +36,11 @@ from .graphics import (Batch, apply_matte, BitmapCompositing, BitmapWindow, Erro
                        RoundCornersMode, flow_bitmap_bgra_clear_around_rounded_corners,
                        FillRect, CopyRectToCanvas, ExpandCanvas, EnableTransparency, new_canvas, watermark_red_dot, region, region_percent,
                        ApplyOrientation, Rotate90, Rotate180, Rotate270, FlipH, FlipV, Transpose, orientation_of, riapi_rotate_steps,
-                       riapi_flip_steps, apply_orientation, oriented_source_window, ColorMatrixSrgb, ColorFilterSrgb, WhiteBalanceHistogramAreaThresholdSrgb,
-                       riapi_color_steps, Watermark, WatermarkConstraintBox, WatermarkConstraintMode, ConstraintGravity, WatermarkDraw,
+                       riapi_flip_steps, apply_orientation, oriented_source_window, oriented_source_rect, ColorMatrixSrgb, ColorFilterSrgb,
+                       WhiteBalanceHistogramAreaThresholdSrgb, riapi_color_steps, Watermark, WatermarkConstraintBox, WatermarkConstraintMode, ConstraintGravity, WatermarkDraw,
                        process_constraint, watermark_layout, riapi_watermark_placement, PixelRows, RgbToBgra, RgbaToBgra, GrayToBgra,
                        GrayAlphaToBgra, BgraToRgb, pixel_op_for, CropWhitespace, riapi_trim_steps, crop_whitespace_bounds)
-from ._lib import LIB_PATH, ResampleDesc, RowsResampleDesc, lib
+from ._lib import LIB_PATH, ResampleDesc, RowsOrientedResampleDesc, RowsResampleDesc, lib
 
 __all__ = [
     "Batch", "apply_matte", "BitmapCompositing", "BitmapWindow", "ErrorKind", "Filter", "FlowError", "ScaleAndRenderParams",
@@ -49,8 +50,9 @@ __all__ = [
     "RoundCornersMode", "flow_bitmap_bgra_clear_around_rounded_corners",
     "FillRect", "CopyRectToCanvas", "ExpandCanvas", "EnableTransparency", "new_canvas", "watermark_red_dot", "region", "region_percent",
     "ApplyOrientation", "Rotate90", "Rotate180", "Rotate270", "FlipH", "FlipV", "Transpose", "orientation_of", "riapi_rotate_steps",
-    "riapi_flip_steps", "apply_orientation", "oriented_source_window", "ColorMatrixSrgb", "ColorFilterSrgb", "WhiteBalanceHistogramAreaThresholdSrgb",
+    "riapi_flip_steps", "apply_orientation", "oriented_source_window", "oriented_source_rect", "ColorMatrixSrgb", "ColorFilterSrgb", "WhiteBalanceHistogramAreaThresholdSrgb",
     "riapi_color_steps", "Watermark", "WatermarkConstraintBox", "WatermarkConstraintMode", "ConstraintGravity", "WatermarkDraw",
     "process_constraint", "watermark_layout", "riapi_watermark_placement", "PixelRows", "RgbToBgra", "RgbaToBgra", "GrayToBgra",
-    "GrayAlphaToBgra", "BgraToRgb", "pixel_op_for", "CropWhitespace", "riapi_trim_steps", "crop_whitespace_bounds", "LIB_PATH", "ResampleDesc", "RowsResampleDesc", "lib",
+    "GrayAlphaToBgra", "BgraToRgb", "pixel_op_for", "CropWhitespace", "riapi_trim_steps", "crop_whitespace_bounds", "LIB_PATH", "ResampleDesc", "RowsOrientedResampleDesc",
+    "RowsResampleDesc", "lib",
 ]

@@ -23,6 +23,7 @@ SYMBOLS = [
     "ifb200_block_scale_u8", "ifb200_batch_block_scale", "ifb200_round_corners_bgra8", "ifb200_batch_round_corners",
     "ifb200_batch_canvas", "ifb200_batch_orient", "ifb200_batch_color_chain", "ifb200_batch_watermark",
     "ifb200_batch_pixel_convert", "ifb200_batch_enqueue_oriented", "ifb200_batch_enqueue_rows", "ifb200_batch_detect_content_many",
+    "ifb200_batch_enqueue_rows_oriented",
 ]
 
 
@@ -46,6 +47,11 @@ class OrientedResampleDesc(C.Structure):
 class RowsResampleDesc(C.Structure):
     """struct ifb200_rows_resample_desc"""
     _fields_ = [("draw", ResampleDesc), ("format", C.c_int32)]
+
+
+class RowsOrientedResampleDesc(C.Structure):
+    """struct ifb200_rows_oriented_resample_desc"""
+    _fields_ = [("draw", ResampleDesc), ("format", C.c_int32), ("orientation", C.c_int32)]
 
 
 class RoundCornersDesc(C.Structure):
@@ -179,6 +185,8 @@ def lib() -> C.CDLL:
     L.ifb200_batch_enqueue_oriented.restype = C.c_int
     L.ifb200_batch_enqueue_rows.argtypes = [C.c_void_p, C.POINTER(RowsResampleDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_enqueue_rows.restype = C.c_int
+    L.ifb200_batch_enqueue_rows_oriented.argtypes = [C.c_void_p, C.POINTER(RowsOrientedResampleDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
+    L.ifb200_batch_enqueue_rows_oriented.restype = C.c_int
     L.ifb200_batch_color_matrix.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, f32p, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_color_matrix.restype = C.c_int
     L.ifb200_batch_sync.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]

@@ -412,9 +412,13 @@ int hv_cols(int av, int ch, int option);
 // ------------------------------------------------------------------------------------------------
 // ring kernel dispatch table
 using HvFn = void (*)(const JobDev*, const HvTmap*, Tables, HvPlanDev, uint32_t, uint32_t*);
-// fn[ORI][EPI] reads BGRA frames, rows[SRC - 1][EPI] the rows of ifb200_batch_enqueue_rows (HV_SRC_RGBA, HV_SRC_RGB24); EPI: general,
-// simple + linear, simple + sRGB
-struct HvEntry { int av, ch; HvFn fn[3][3]; int threads, warps, max_cols, ng; uint32_t (*smem)(uint32_t); HvFn rows[2][3]; };
+// fn[ORI][EPI] reads BGRA frames, rows[SRC - 1][EPI] the rows of ifb200_batch_enqueue_rows (HV_SRC_RGBA, HV_SRC_RGB24),
+// rows_ori[SRC - 1][ORI - 1][EPI] those of ifb200_batch_enqueue_rows_oriented; EPI: general, simple + linear, simple + sRGB.  A null
+// entry is a form that is not compiled (its jobs take the generic pair).
+struct HvEntry { int av, ch; HvFn fn[3][3]; int threads, warps, max_cols, ng; uint32_t (*smem)(uint32_t); HvFn rows[2][3]; HvFn rows_ori[2][2][3]; };
+HvFn hv_form(const HvEntry* e, int ori, int src, int epi) {
+    return src == HV_SRC_BGRA ? e->fn[ori][epi] : ori == HV_ORI_NONE ? e->rows[src - 1][epi] : e->rows_ori[src - 1][ori - 1][epi];
+}
 template <int AV, int CH> uint32_t hv_smem_bytes(uint32_t sb_low16) { return hv_total_bytes<AV, CH>(sb_low16); }
 #define IFB_HV_EPI(AV_, CH_, O_) {hv_ring_kernel<AV_, CH_, 0, O_>, hv_ring_kernel<AV_, CH_, 1, O_>, hv_ring_kernel<AV_, CH_, 2, O_>}
 // The RGB24 form with the general store epilogue at ring depth 6 and three channels spills (one register over the 128 of 16 warps):
@@ -424,9 +428,16 @@ template <> constexpr HvFn kRgb24General<6, 3> = nullptr;
 #define IFB_HV_SRC(AV_, CH_) {{hv_ring_kernel<AV_, CH_, 0, HV_ORI_NONE, HV_SRC_RGBA>, hv_ring_kernel<AV_, CH_, 1, HV_ORI_NONE, HV_SRC_RGBA>, \
                                hv_ring_kernel<AV_, CH_, 2, HV_ORI_NONE, HV_SRC_RGBA>}, \
                               {kRgb24General<AV_, CH_>, hv_ring_kernel<AV_, CH_, 1, HV_ORI_NONE, HV_SRC_RGB24>, hv_ring_kernel<AV_, CH_, 2, HV_ORI_NONE, HV_SRC_RGB24>}}
+template <int AV, int CH, int EPI, int ORI, int SRC> constexpr HvFn kRowsOriented = hv_ring_kernel<AV, CH, EPI, ORI, SRC>;
+// The RGB24 flip forms at ring depth 6 with three channels spill 4 bytes with the general and the linear store epilogues: not compiled
+template <> constexpr HvFn kRowsOriented<6, 3, 0, HV_ORI_FLIP, HV_SRC_RGB24> = nullptr;
+template <> constexpr HvFn kRowsOriented<6, 3, 1, HV_ORI_FLIP, HV_SRC_RGB24> = nullptr;
+#define IFB_HV_RO(AV_, CH_, O_, S_) {kRowsOriented<AV_, CH_, 0, O_, S_>, kRowsOriented<AV_, CH_, 1, O_, S_>, kRowsOriented<AV_, CH_, 2, O_, S_>}
+#define IFB_HV_ROWS_ORI(AV_, CH_) {{IFB_HV_RO(AV_, CH_, HV_ORI_FLIP, HV_SRC_RGBA), IFB_HV_RO(AV_, CH_, HV_ORI_TRANSPOSE, HV_SRC_RGBA)}, \
+                                   {IFB_HV_RO(AV_, CH_, HV_ORI_FLIP, HV_SRC_RGB24), IFB_HV_RO(AV_, CH_, HV_ORI_TRANSPOSE, HV_SRC_RGB24)}}
 #define IFB_HV(AV_, CH_) {AV_, CH_, {IFB_HV_EPI(AV_, CH_, HV_ORI_NONE), IFB_HV_EPI(AV_, CH_, HV_ORI_FLIP), IFB_HV_EPI(AV_, CH_, HV_ORI_TRANSPOSE)}, \
                           HvCfg<AV_, CH_>::kThreads, HvCfg<AV_, CH_>::kWarps, HvCfg<AV_, CH_>::kMaxCols, HvCfg<AV_, CH_>::kNG, hv_smem_bytes<AV_, CH_>, \
-                          IFB_HV_SRC(AV_, CH_)}
+                          IFB_HV_SRC(AV_, CH_), IFB_HV_ROWS_ORI(AV_, CH_)}
 const HvEntry kHv[] = {IFB_HV(4, 3), IFB_HV(4, 4), IFB_HV(6, 3), IFB_HV(6, 4)};
 const HvEntry* find_hv(int av, int ch) {
     for (const auto& e : kHv) if (e.av == av && e.ch == ch) return &e;
@@ -760,7 +771,8 @@ void host_tables() {
 // (the oriented kernel of flags 5..8): box 32 x 16, no swizzle.  d is the window as stored.
 // The base is aligned down to 16 bytes (a window may start at any pixel: bitmaps.rs:413-431); the kernel adds the 0..3 pixels
 // it was moved by to its x coordinates.  `bytes` (RGB24 rows of ifb200_batch_enqueue_rows): u8 elements, the 0..15 bytes between
-// the base and d.in plus 3 in_w bytes per row, box 64 x 32, SWIZZLE_64B; *xoff_out is then those 0..15 bytes.
+// the base and d.in plus 3 in_w bytes per row, box 64 x 32, SWIZZLE_64B (both: box 128 bytes x 16 rows, no swizzle); *xoff_out is
+// then those 0..15 bytes.
 const HvTmap& tmap_for(ifb200_batch* b, const ifb200_resample_desc& d, uint32_t* xoff_out, bool transposed = false, bool bytes = false) {
     const uintptr_t addr = (uintptr_t)d.in;
     const uintptr_t base = addr & ~(uintptr_t)15;
@@ -774,7 +786,7 @@ const HvTmap& tmap_for(ifb200_batch* b, const ifb200_resample_desc& d, uint32_t*
     CUtensorMap tm;
     const cuuint64_t dims[2] = {(cuuint64_t)w, (cuuint64_t)d.in_h};
     const cuuint64_t strides[1] = {(cuuint64_t)d.in_stride};
-    const cuuint32_t box[2] = {bytes ? 64u : transposed ? 32u : 16u, transposed ? 16u : 32u};
+    const cuuint32_t box[2] = {bytes ? (transposed ? 128u : 64u) : transposed ? 32u : 16u, transposed ? 16u : 32u};
     const cuuint32_t estr[2] = {1u, 1u};
     // L2 promotion: how much of a line a 64-byte box row pulls into L2 (IFB200_DEBUG_L2_PROMOTION = 0 / 64 / 128 / 256 for experiments)
     static const CUtensorMapL2promotion promo = [] {
@@ -811,6 +823,7 @@ uint32_t ori_flips(int flag) {
 // pair with the oriented H pass (there is no oriented tile kernel).
 // src != nullptr (enqueue_rows_locked): descs[i].in holds rows of format src[i] (HV_SRC_RGBA / HV_SRC_RGB24), checked by the
 // caller; these jobs take the ring kernel's row forms or the generic pair with hpass_rows_kernel (there is no tile-kernel form).
+// Both (enqueue_rows_oriented_locked): the ring kernel's oriented row forms or the generic pair with hpass_oriented_kernel<TR, BPP>.
 void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n, cudaStream_t st, const int32_t* ori = nullptr,
                     const int32_t* src = nullptr) {
     if (!descs && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
@@ -840,14 +853,14 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
         // W - 32 - y (flags 7, 8), so the stored width W (in_w, or in_h of the oriented plan for 5..8) must be a multiple of four
         if (oc != HV_ORI_NONE && (ori_flips(ori[i]) & JF_FLIP_X) && ((oc == HV_ORI_TRANSPOSE ? p.in_h : p.in_w) & 3u)) ring = false;
         // rows: up-scales and 1:1 take the generic pair; RGB24 rows may start at any byte (the box origins are aligned below the
-        // window's first byte), so only the pitch must be a multiple of 16 bytes
+        // window's first byte), so only the pitch must be a multiple of 16 bytes -- also with source x reversed, for any width
         const int sf = src ? src[i] : HV_SRC_BGRA;
         if (sf != HV_SRC_BGRA) {
             if (sf == HV_SRC_RGB24) ring = p.hv_ok && b->ring_ok && !b->force_generic && (d.in_stride % 16 == 0);
             if (upscale) ring = false;
         }
         const bool simple = d.compose == IFB200_REPLACE_SELF && !d.color_matrix;   // store epilogue without composite / matrix code
-        if (ring && sf != HV_SRC_BGRA && !find_hv(p.av, ch)->rows[sf - 1][simple ? 1 : 0]) ring = false;   // a form not compiled
+        if (ring && sf != HV_SRC_BGRA && !hv_form(find_hv(p.av, ch), oc, sf, simple ? (d.linear ? 1 : 2) : 0)) ring = false;   // a form not compiled
         if (ring && !(p.tile_ok && upscale) && !hv_host_ready(p, hv_cols(p.av, ch, b->strip_cols))) ring = false;   // windows wider than the weight table
         // the ring kernel streams every source row once and wins whenever rows outnumber outputs (down-scales);
         // for up-scales / 1:1 the tile kernel does less work per source pixel
@@ -1014,7 +1027,7 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
             pl.vw = ht.blob.at<float>(ht.o_vw); pl.vdone = ht.blob.at<uint8_t>(ht.o_vdone);
             pl.hw_stride = ht.hw_stride;
             const int epi = g.simple ? ((g.variant & 1) ? 1 : 2) : 0;       // the ring kernel's launches are per working space (variant bit 0 = linear)
-            HvFn fn = g.src != HV_SRC_BGRA ? he->rows[g.src - 1][epi] : he->fn[g.ori][epi];
+            HvFn fn = hv_form(he, g.ori, g.src, epi);
             const size_t smem = he->smem(b->smem_base_low16);
             if (!b->hv_attr_set.count((const void*)fn)) {
                 CUDA_OK(cudaFuncSetAttribute((const void*)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1036,19 +1049,21 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
             AsyncFree inter_guard{inter, st};
             for (size_t off = 0; off < nj; off += chunk) {
                 const size_t cnt = std::min(chunk, nj - off);
-                if (g.src != HV_SRC_BGRA) {
+                if (g.ori == HV_ORI_NONE && g.src != HV_SRC_BGRA) {
                     dim3 gh((p.out_w + 127) / 128, std::min<uint32_t>(p.in_h, 65535u), (unsigned)cnt);
                     if (g.src == HV_SRC_RGB24) hpass_rows_kernel<3><<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_h, p.out_w, inter);
                     else hpass_rows_kernel<4><<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_h, p.out_w, inter);
                 } else if (g.ori == HV_ORI_NONE) {
                     dim3 gh((p.out_w + 127) / 128, std::min<uint32_t>(p.in_h, 65535u), (unsigned)cnt);
                     hpass_generic_kernel<<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_h, p.out_w, inter);
-                } else if (g.ori == HV_ORI_FLIP) {
-                    dim3 gh((p.out_w + 127) / 128, std::min<uint32_t>(p.in_h, 65535u), (unsigned)cnt);
-                    hpass_oriented_kernel<false><<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_w, p.in_h, p.out_w, inter);
-                } else {                                                  // threads along oriented rows = along a source row
-                    dim3 gh((p.in_h + 127) / 128, std::min<uint32_t>(p.out_w, 65535u), (unsigned)cnt);
-                    hpass_oriented_kernel<true><<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_w, p.in_h, p.out_w, inter);
+                } else {
+                    // flips: threads along output columns; transposes: threads along oriented rows = along a source row
+                    const bool tr = g.ori == HV_ORI_TRANSPOSE;
+                    dim3 gh(((tr ? p.in_h : p.out_w) + 127) / 128, std::min<uint32_t>(tr ? p.out_w : p.in_h, 65535u), (unsigned)cnt);
+                    using HFn = void (*)(const JobDev*, Tables, AxisDev, uint32_t, uint32_t, uint32_t, float4*);
+                    static const HFn kOriented[2][3] = {{hpass_oriented_kernel<false>, hpass_oriented_kernel<false, 4>, hpass_oriented_kernel<false, 3>},
+                                                        {hpass_oriented_kernel<true>, hpass_oriented_kernel<true, 4>, hpass_oriented_kernel<true, 3>}};
+                    kOriented[tr][g.src]<<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_w, p.in_h, p.out_w, inter);
                 }
                 CUDA_OK(cudaGetLastError());
                 dim3 gv((p.out_w + 127) / 128, std::min<uint32_t>(p.out_h, 65535u), (unsigned)cnt);
@@ -1062,74 +1077,99 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
     st = user_stream;
 }
 
-// ifb200_batch_enqueue_oriented: every descriptor is checked as stored and every plan (of the oriented geometry) is built before
-// anything is enqueued; then the identity jobs go through enqueue_locked exactly as ifb200_batch_enqueue sends them, and the others
+// The checks of one descriptor of decoder rows (ifb200_batch_enqueue_rows, _rows_oriented), on the rows as stored: its format, the
+// resample's own rules (resample_check, with the rows' rules in place of a BGRA row's), then the rows'.  `what` begins every message,
+// `bgra_entry` is where a Gray8 / GrayAlpha8 job's BGRA frame goes instead.  Returns the job's HV_SRC_*.
+int check_rows(const ifb200_resample_desc& r, int32_t f, size_t i, const char* what, const char* bgra_entry) {
+    if (f == IFB200_PIXEL_GRAY_TO_BGRA || f == IFB200_PIXEL_GRAY_ALPHA_TO_BGRA)
+        IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "%s job %zu: format %d (%s) has no resample form; convert the rows with "
+                  "ifb200_batch_pixel_convert, then resample the BGRA frame with %s", what, i, (int)f,
+                  f == IFB200_PIXEL_GRAY_TO_BGRA ? "Gray8" : "GrayAlpha8", bgra_entry);
+    if (f != IFB200_PIXEL_RGB24_TO_BGRA && f != IFB200_PIXEL_RGBA_TO_BGRA)
+        IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "%s job %zu: format %d is not IFB200_PIXEL_RGB24_TO_BGRA (0) or "
+                  "IFB200_PIXEL_RGBA_TO_BGRA (1)", what, i, (int)f);
+    ifb200_resample_desc c = r;                                           // every rule but the row's
+    c.in_w = r.in_w ? 1u : 0u; c.in_stride = 4u;
+    int code = 0;
+    const std::string why = ifb::resample_check(c, &code);
+    if (!why.empty()) IFB_THROW(code, "%s job %zu: %s", what, i, why.c_str());
+    const uint32_t bpp = f == IFB200_PIXEL_RGB24_TO_BGRA ? 3u : 4u;
+    if (r.in_stride < (uint64_t)r.in_w * bpp)
+        IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "%s job %zu: stride %u smaller than a row of %u %s pixels", what, i, r.in_stride,
+                  r.in_w, bpp == 3u ? "RGB24" : "RGBA32");
+    if (bpp == 4u && (((uintptr_t)r.in & 3) || (r.in_stride & 3)))
+        IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "%s job %zu: RGBA32 rows need a 4-byte aligned pointer and stride", what, i);
+    return bpp == 3u ? HV_SRC_RGB24 : HV_SRC_RGBA;
+}
+
+// n checked jobs of stored windows (BGRA frames when src is null, else rows of formats src[i]) with EXIF flags orientation[i]
+// (null: all identity): every plan -- of the oriented geometry, in_w and in_h swapped for 5..8 -- is built before anything is
+// enqueued; then the identity jobs go through enqueue_locked exactly as ifb200_batch_enqueue / _rows send them, and the others
 // through its oriented forms.
-void enqueue_oriented_locked(ifb200_batch* b, const ifb200_oriented_resample_desc* d, size_t n, cudaStream_t st) {
-    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
-    if (n == 0) return;
-    for (size_t i = 0; i < n; ++i) {
-        int code = 0;
-        const std::string why = ifb::resample_check(d[i].draw, &code);
-        if (!why.empty()) IFB_THROW(code, "oriented resample job %zu: %s", i, why.c_str());
-    }
+void enqueue_oriented_split(ifb200_batch* b, const ifb200_resample_desc* draws, const int32_t* orientation, const int32_t* src, size_t n,
+                            cudaStream_t st) {
     std::vector<ifb200_resample_desc> plain, turned;
-    std::vector<int32_t> flags;
+    std::vector<int32_t> flags, plain_src, turned_src;
     for (size_t i = 0; i < n; ++i) {
-        const int32_t o = d[i].orientation;
-        if (ori_class(o) == HV_ORI_NONE) { plain.push_back(d[i].draw); continue; }
-        ifb200_resample_desc od = d[i].draw;
+        const int32_t o = orientation ? orientation[i] : 1;
+        const int32_t s = src ? src[i] : HV_SRC_BGRA;
+        if (ori_class(o) == HV_ORI_NONE) { plain.push_back(draws[i]); plain_src.push_back(s); continue; }
+        ifb200_resample_desc od = draws[i];
         if (ori_class(o) == HV_ORI_TRANSPOSE) std::swap(od.in_w, od.in_h);
         turned.push_back(od);
+        turned_src.push_back(s);
         flags.push_back(o);
     }
     {
         Tick tk(b->prof.plans);
+        // BGRA identity jobs are checked and planned by enqueue_locked itself, as ifb200_batch_enqueue does it
+        if (src) { b->prebuild_plans(plain.data(), plain.size()); for (const auto& r : plain) b->plan_for(r); }   // may throw: nothing enqueued yet
         b->prebuild_plans(turned.data(), turned.size());
-        for (const auto& od : turned) b->plan_for(od);                   // may throw: nothing enqueued yet
+        for (const auto& od : turned) b->plan_for(od);
     }
-    enqueue_locked(b, plain.data(), plain.size(), st);
-    enqueue_locked(b, turned.data(), turned.size(), st, flags.data());
+    enqueue_locked(b, plain.data(), plain.size(), st, nullptr, src ? plain_src.data() : nullptr);
+    enqueue_locked(b, turned.data(), turned.size(), st, flags.data(), src ? turned_src.data() : nullptr);
 }
 
-// ifb200_batch_enqueue_rows: every descriptor is checked -- its format, the resample's own rules (resample_check, with the rows'
-// rules in place of a BGRA row's), then the rows' -- and every plan built before anything is enqueued; then all jobs go through
-// enqueue_locked's row forms.
+// ifb200_batch_enqueue_oriented: every descriptor is checked as stored, then enqueue_oriented_split.
+void enqueue_oriented_locked(ifb200_batch* b, const ifb200_oriented_resample_desc* d, size_t n, cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    if (n == 0) return;
+    std::vector<ifb200_resample_desc> draws(n);
+    std::vector<int32_t> flags(n);
+    for (size_t i = 0; i < n; ++i) {
+        int code = 0;
+        const std::string why = ifb::resample_check(d[i].draw, &code);
+        if (!why.empty()) IFB_THROW(code, "oriented resample job %zu: %s", i, why.c_str());
+        draws[i] = d[i].draw; flags[i] = d[i].orientation;
+    }
+    enqueue_oriented_split(b, draws.data(), flags.data(), nullptr, n, st);
+}
+
+// ifb200_batch_enqueue_rows: every descriptor is checked (check_rows), then every job goes through enqueue_locked's row forms.
 void enqueue_rows_locked(ifb200_batch* b, const ifb200_rows_resample_desc* d, size_t n, cudaStream_t st) {
     if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
     if (n == 0) return;
     std::vector<ifb200_resample_desc> draws(n);
     std::vector<int32_t> src(n);
     for (size_t i = 0; i < n; ++i) {
-        const ifb200_resample_desc& r = d[i].draw;
-        const int32_t f = d[i].format;
-        if (f == IFB200_PIXEL_GRAY_TO_BGRA || f == IFB200_PIXEL_GRAY_ALPHA_TO_BGRA)
-            IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "rows resample job %zu: format %d (%s) has no resample form; convert the rows with "
-                      "ifb200_batch_pixel_convert, then resample the BGRA frame with ifb200_batch_enqueue", i, (int)f,
-                      f == IFB200_PIXEL_GRAY_TO_BGRA ? "Gray8" : "GrayAlpha8");
-        if (f != IFB200_PIXEL_RGB24_TO_BGRA && f != IFB200_PIXEL_RGBA_TO_BGRA)
-            IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "rows resample job %zu: format %d is not IFB200_PIXEL_RGB24_TO_BGRA (0) or "
-                      "IFB200_PIXEL_RGBA_TO_BGRA (1)", i, (int)f);
-        ifb200_resample_desc c = r;                                       // every rule but the row's
-        c.in_w = r.in_w ? 1u : 0u; c.in_stride = 4u;
-        int code = 0;
-        const std::string why = ifb::resample_check(c, &code);
-        if (!why.empty()) IFB_THROW(code, "rows resample job %zu: %s", i, why.c_str());
-        const uint32_t bpp = f == IFB200_PIXEL_RGB24_TO_BGRA ? 3u : 4u;
-        if (r.in_stride < (uint64_t)r.in_w * bpp)
-            IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "rows resample job %zu: stride %u smaller than a row of %u %s pixels", i, r.in_stride,
-                      r.in_w, bpp == 3u ? "RGB24" : "RGBA32");
-        if (bpp == 4u && (((uintptr_t)r.in & 3) || (r.in_stride & 3)))
-            IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "rows resample job %zu: RGBA32 rows need a 4-byte aligned pointer and stride", i);
-        draws[i] = r;
-        src[i] = bpp == 3u ? HV_SRC_RGB24 : HV_SRC_RGBA;
+        src[i] = check_rows(d[i].draw, d[i].format, i, "rows resample", "ifb200_batch_enqueue");
+        draws[i] = d[i].draw;
     }
-    {
-        Tick tk(b->prof.plans);
-        b->prebuild_plans(draws.data(), n);
-        for (const auto& r : draws) b->plan_for(r);                      // may throw: nothing enqueued yet
+    enqueue_oriented_split(b, draws.data(), nullptr, src.data(), n, st);
+}
+
+// ifb200_batch_enqueue_rows_oriented: every descriptor is checked on the stored rows (check_rows), then enqueue_oriented_split.
+void enqueue_rows_oriented_locked(ifb200_batch* b, const ifb200_rows_oriented_resample_desc* d, size_t n, cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    if (n == 0) return;
+    std::vector<ifb200_resample_desc> draws(n);
+    std::vector<int32_t> src(n), flags(n);
+    for (size_t i = 0; i < n; ++i) {
+        src[i] = check_rows(d[i].draw, d[i].format, i, "oriented rows resample", "ifb200_batch_enqueue_oriented");
+        draws[i] = d[i].draw; flags[i] = d[i].orientation;
     }
-    enqueue_locked(b, draws.data(), n, st, nullptr, src.data());
+    enqueue_oriented_split(b, draws.data(), flags.data(), src.data(), n, st);
 }
 
 // The argument checks of a BGRA window, shared by the device and the host-buffer form of each operation: a null pointer, or a stride
@@ -1936,6 +1976,10 @@ int ifb200_batch_enqueue_oriented(ifb200_batch* b, const ifb200_oriented_resampl
 
 int ifb200_batch_enqueue_rows(ifb200_batch* b, const ifb200_rows_resample_desc* d, size_t n, void* stream, char* err, size_t cap) {
     return with_batch(b, stream, err, cap, [&](cudaStream_t st) { enqueue_rows_locked(b, d, n, st); });
+}
+
+int ifb200_batch_enqueue_rows_oriented(ifb200_batch* b, const ifb200_rows_oriented_resample_desc* d, size_t n, void* stream, char* err, size_t cap) {
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { enqueue_rows_oriented_locked(b, d, n, st); });
 }
 
 int ifb200_batch_color_matrix(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, const float m[25],

@@ -61,7 +61,7 @@ struct alignas(64) HvTmap { unsigned char bytes[128]; };              // CUtenso
 enum : int { HV_ORI_NONE = 0, HV_ORI_FLIP = 1, HV_ORI_TRANSPOSE = 2 };
 // The source pixel format an instantiation reads (template parameter SRC, ifb200_batch_enqueue_rows): BGRA32 (0); RGBA32 (1), the
 // same u32 box, the table look-ups taking blue from byte 2 and red from byte 0; RGB24 (2), a UINT8 tensor read in boxes of 64 bytes
-// x 32 rows, 16 pixels (48 bytes) at a constant offset r inside each box.  Only the stored frame (ORI = HV_ORI_NONE) has these forms.
+// x 32 rows, 16 pixels (48 bytes) at a constant offset r inside each box (transposed: boxes of 128 bytes x 16 rows, 32 pixels at r).
 enum : int { HV_SRC_BGRA = 0, HV_SRC_RGBA = 1, HV_SRC_RGB24 = 2 };
 
 #ifndef IFB_HV_MAXCOLS4
@@ -330,11 +330,17 @@ __device__ __forceinline__ uint32_t hv_finish_pixel(float b, float g, float r, f
 // 16-byte aligned and the pixels sit at byte r = (phase + 3x) & 15 of every box row, the same r all along the stream (48 = 0 mod
 // 16; r + 48 <= 63).  A lane's chunk k is bytes r + 12k .. r + 12k + 11 of its row: four 4-byte loads (words r/4 + 3k ..) and byte
 // permutes give its four pixels as words with red in byte 0, green in byte 1, blue in byte 2 (byte 3 unused: alpha is 255).
+// Both together (ifb200_batch_enqueue_rows_oriented): RGBA32 is the BGRA oriented form with the look-ups' blue and red swapped.  RGB24
+// flips keep the 64-byte box; a backwards stream axis fetches far-end boxes at byte phase + 3 (W - 16 - x) aligned down to 16, 48
+// bytes lower each step, so that r stays constant again, and reads chunk 3 - k, its four pixels reversed; a backwards lane axis gives
+// lane l box row 31 - l with that row's swizzle.  RGB24 transposes read boxes of 128 bytes x 16 source rows, unswizzled, whose origin
+// is phase + 3 x0 aligned down to 16 (x0: the source column of box column 0; 32 columns are 96 bytes, + up to 15 of r): lane l (or
+// 31 - l) finds its pixel at byte r + 3 l of each box row, two 4-byte loads and a byte permute; the 32 lanes' loads fall in 24
+// consecutive words.  Byte-aligned origins need neither the band's early start of the BGRA transposes nor a width rule.
 template <int AV, int CH, int EPI, int ORI = HV_ORI_NONE, int SRC = HV_SRC_BGRA>
 __global__ void __launch_bounds__(HvCfg<AV, CH>::kThreads, 1)
 hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps, Tables tb, HvPlanDev pl, uint32_t n_jobs,
                uint32_t* __restrict__ counters) {
-    static_assert(SRC == HV_SRC_BGRA || ORI == HV_ORI_NONE, "row formats are read without orientation");
     using C = HvCfg<AV, CH>;
     constexpr int AVP = C::kAvp, NG = C::kNG, NP = C::kNP, S = C::kStages, CG = C::kCG;
     constexpr uint32_t kRec = (uint32_t)AVP * 4u;                          // bytes per H weight record (one source column)
@@ -421,7 +427,7 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
             // reversed lanes here only when the stored width is a multiple of four, so that W - 32 - row is one too).  The rows added
             // complete only output rows above the band (never stored), which the V pass then starts with: `early` of them.
             uint32_t early = 0;
-            if constexpr (ORI == HV_ORI_TRANSPOSE) {
+            if constexpr (ORI == HV_ORI_TRANSPOSE && SRC != HV_SRC_RGB24) {
                 const int a = bJ0 & 3;
                 for (int j = bJ0 - a; j < bJ0; ++j) early += (uint32_t)hv::ldg(pl.vdone + j);
                 bJ0 -= a; bNr += a;
@@ -431,8 +437,13 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
             const int nrb = (bNr + 31) >> 5;
             // where the stream starts in the tensor: pixel sK0 + xoff; RGB24, byte phase + 3 sK0 (its boxes at x & ~15, its pixels at
             // r = x_origin & 15 of every box row: no register beyond the BGRA form's, which is at the register budget)
-            constexpr int kBoxX = SRC == HV_SRC_RGB24 ? 48 : 16;               // tensor elements per 16 pixels
-            const int x_origin = SRC == HV_SRC_RGB24 ? (int)uni(job.in_xoff) + 3 * sK0 : sK0 + (int)uni(job.in_xoff);
+            // RGB24 flips with the stream backwards: the far-end byte of the first box (issue() walks down from it); RGB24 transposes:
+            // the stream runs over source rows, which have no phase
+            constexpr bool kBytesX = SRC == HV_SRC_RGB24 && ORI != HV_ORI_TRANSPOSE;
+            constexpr int kBoxX = kBytesX ? 48 : 16;                           // tensor elements per 16 pixels
+            const int x_origin = kBytesX ? (int)uni(job.in_xoff) + 3 * (ORI == HV_ORI_FLIP && (flags & JF_FLIP_X) ? (int)pl.in_w - 16 - sK0 : sK0)
+                                         : sK0 + (SRC == HV_SRC_RGB24 ? 0 : (int)uni(job.in_xoff));
+            const int t_phase = SRC == HV_SRC_RGB24 && ORI == HV_ORI_TRANSPOSE ? (int)uni(job.in_xoff) : 0;   // RGB24 transposes: the rows' phase
 
             // ---- TMA pipeline state: boxes are fetched row block by row block, left to right
             const int x_end = x_origin + nst * kBoxX;
@@ -446,6 +457,15 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
                         hv::tma_load_box(stb + (uint32_t)is_s * C::kStageBytes, tm, (tma_x & ~15) + (int)zero_dep, tma_y, bar);
                     } else if constexpr (ORI == HV_ORI_NONE) {
                         hv::tma_load_box(stb + (uint32_t)is_s * C::kStageBytes, tm, tma_x + (int)zero_dep, tma_y, bar);
+                    } else if constexpr (SRC == HV_SRC_RGB24) {
+                        const bool rs = (flags & (ORI == HV_ORI_FLIP ? JF_FLIP_X : JF_FLIP_Y)) != 0u, rl = (flags & (ORI == HV_ORI_FLIP ? JF_FLIP_Y : JF_FLIP_X)) != 0u;
+                        const int l0 = rl ? (int)pl.in_h - 32 - tma_y : tma_y;
+                        if constexpr (ORI == HV_ORI_FLIP) {                // byte tma_x, or down from x_origin (the far end) when reversed
+                            hv::tma_load_box(stb + (uint32_t)is_s * C::kStageBytes, tm, ((rs ? 2 * x_origin - tma_x : tma_x) & ~15) + (int)zero_dep, l0, bar);
+                        } else {                                           // source columns l0 .. l0 + 31 of source rows s0 .. s0 + 15
+                            const int s0 = rs ? (int)pl.in_w - 16 - tma_x : tma_x;
+                            hv::tma_load_box(stb + (uint32_t)is_s * C::kStageBytes, tm, ((t_phase + 3 * l0) & ~15) + (int)zero_dep, s0, bar);
+                        }
                     } else {
                         // the box of oriented columns [tma_x, +16) x rows [tma_y, +32) in the stored frame (pl.in_w x pl.in_h is the
                         // oriented size: the stored frame is in_w x in_h for flips, in_h x in_w for transposes)
@@ -470,8 +490,14 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
             // Flips (s = 4): row lrow at lrow * 64, chunk (k ^ 3 if reversed) of it at (that << 4) ^ the row's 64-byte swizzle.
             // Transposes (s = 9): column lrow at lrow * 4 in box rows 4k .. 4k + 3 (15 - 4k down to 12 - 4k if reversed; 15 - x ==
             // 15 ^ x for x <= 15).  The parts occupy disjoint bits, so they combine by xor.
-            const uint32_t lo = ORI == HV_ORI_FLIP ? (lrow * 64u) | ((((lrow >> 1) & 3u) << 4) ^ (rev_s ? 0x30u : 0u))
-                                                   : (lrow * 4u) | (rev_s ? 15u << 7 : 0u);
+            // RGB24 flips: the row and its swizzle only (a reversed stream reads chunk 3 - k).  RGB24 transposes: the first of the lane's
+            // two words around byte r + 3 lrow, r_t = the byte of box column 0 in a box row (the same for every row block of the band:
+            // 32 columns are 96 bytes), and tsel the byte permute that starts at the pixel.
+            const uint32_t r_t = SRC == HV_SRC_RGB24 && ORI == HV_ORI_TRANSPOSE ? ((uint32_t)t_phase + 3u * (uint32_t)(rev_l ? (int)pl.in_h - 32 - bJ0 : bJ0)) & 15u : 0u;
+            const uint32_t lo = ORI == HV_ORI_FLIP ? (lrow * 64u) | ((((lrow >> 1) & 3u) << 4) ^ (rev_s && SRC != HV_SRC_RGB24 ? 0x30u : 0u))
+                              : SRC == HV_SRC_RGB24 ? ((r_t + 3u * lrow) & ~3u) | (rev_s ? 15u << 7 : 0u)
+                                                    : (lrow * 4u) | (rev_s ? 15u << 7 : 0u);
+            const uint32_t tsel = 0x3210u + 0x1111u * ((r_t + 3u * lrow) & 3u);
             // chunk k (four oriented columns) of this lane's row in the stage at sb_ (the stage, + lane * 64 for the stored frame)
             auto chunk = [&](const uint32_t sb_, const uint32_t k_) -> uint4 {
                 if constexpr (ORI == HV_ORI_NONE && SRC == HV_SRC_RGB24) {
@@ -485,6 +511,19 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
                     return make_uint4(y0, hv::prmt(y0, y1, 0x6543u), hv::prmt(y1, y2, 0x5432u), y2 >> 8);
                 } else if constexpr (ORI == HV_ORI_NONE) {
                     return hv::lds_u32x4(sb_ + ((k_ << 4) ^ swz));
+                } else if constexpr (ORI == HV_ORI_FLIP && SRC == HV_SRC_RGB24) {
+                    // the stored form's chunk (3 - k when reversed) from row offset lo, its pixels reversed
+                    const uint32_t a = ((uint32_t)x_origin & 12u) + 12u * (rev_s ? 3u - k_ : k_), fsel = 0x3210u + 0x1111u * ((uint32_t)x_origin & 3u);
+                    const uint32_t x0 = hv::lds_u32(sb_ + (a ^ lo)), x1 = hv::lds_u32(sb_ + ((a + 4u) ^ lo));
+                    const uint32_t x2 = hv::lds_u32(sb_ + ((a + 8u) ^ lo)), x3 = hv::lds_u32(sb_ + ((a + 12u) ^ lo));
+                    const uint32_t y0 = hv::prmt(x0, x1, fsel), y1 = hv::prmt(x1, x2, fsel), y2 = hv::prmt(x2, x3, fsel);
+                    const uint32_t p1 = hv::prmt(y0, y1, 0x6543u), p2 = hv::prmt(y1, y2, 0x5432u), p3 = y2 >> 8;
+                    return rev_s ? make_uint4(p3, p2, p1, y0) : make_uint4(y0, p1, p2, p3);
+                } else if constexpr (ORI == HV_ORI_TRANSPOSE && SRC == HV_SRC_RGB24) {
+                    const uint32_t a = sb_ + ((k_ << 9) ^ lo);
+                    const uint32_t step = rev_s ? 0u - 128u : 128u;
+                    auto px = [&](const uint32_t q) { return hv::prmt(hv::lds_u32(a + q), hv::lds_u32(a + q + 4u), tsel); };
+                    return make_uint4(px(0u), px(step), px(2u * step), px(3u * step));
                 } else if constexpr (ORI == HV_ORI_FLIP) {
                     const uint4 v = hv::lds_u32x4(sb_ + ((k_ << 4) ^ lo));
                     return (flags & JF_FLIP_X) ? make_uint4(v.w, v.z, v.y, v.x) : v;

@@ -68,9 +68,17 @@ __global__ void __launch_bounds__(128) hpass_generic_kernel(const JobDev* __rest
 // column X of ORIENTED row j, each tap read from the stored window through the orientation (in_w x in_h is the oriented size;
 // JF_FLIP_X / JF_FLIP_Y of the job).  Writes the intermediate vpass_generic_kernel reads.  TR (flags 5..8): thread = oriented row,
 // blockIdx.y = output column, so that a warp's loads of one tap are consecutive pixels of one source row.
-template <bool TR>
+// BPP 0: BGRA frames; 3 / 4: decoder rows (ifb200_batch_enqueue_rows_oriented), each tap read and converted as hpass_rows_kernel<BPP>
+// reads it (rows_tap_bgra, below).
+template <int BPP>                                               // one tap of decoder rows at p as a BGRA word
+__device__ __forceinline__ uint32_t rows_tap_bgra(const uint8_t* p) {
+    if constexpr (BPP == 3) return (uint32_t)__ldg(p + 2) | ((uint32_t)__ldg(p + 1) << 8) | ((uint32_t)__ldg(p) << 16) | 0xff000000u;
+    else return __byte_perm(__ldg(reinterpret_cast<const uint32_t*>(p)), 0u, 0x3012);
+}
+template <bool TR, int BPP = 0>
 __global__ void __launch_bounds__(128) hpass_oriented_kernel(const JobDev* __restrict__ jobs, Tables tb, AxisDev ah, uint32_t in_w,
                                                              uint32_t in_h, uint32_t out_w, float4* __restrict__ inter) {
+    constexpr size_t kPx = BPP == 0 ? 4 : BPP;                   // bytes per stored pixel
     const JobDev& job = jobs[blockIdx.z];
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (TR ? in_h : out_w)) return;
@@ -83,15 +91,17 @@ __global__ void __launch_bounds__(128) hpass_oriented_kernel(const JobDev* __res
         // oriented (k, j) -> stored pixel: flags 1..4 (k or w-1-k, j or h-1-j), 5..8 (j or w-1-j, k or h-1-k), w x h as stored
         // (= in_w x in_h, or in_h x in_w); `line` is where oriented row j lies in the stored window, `step` the bytes between taps
         const uint32_t jj = (TR ? fx : fy) ? in_h - 1u - j : j;
-        const uint8_t* line = TR ? job.in + (size_t)jj * 4 : job.in + (size_t)jj * job.in_stride;
-        const size_t step = TR ? job.in_stride : 4;
+        const uint8_t* line = TR ? job.in + (size_t)jj * kPx : job.in + (size_t)jj * job.in_stride;
+        const size_t step = TR ? job.in_stride : kPx;
         const bool rev = TR ? fy : fx;           // the taps walk the stored axis backwards
         const uint32_t l = ah.left[X], r = ah.right[X];
         const float* __restrict__ w = ah.w + ah.off[X];
         float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
         for (uint32_t k = l; k <= r; ++k) {
             const uint32_t ks = rev ? in_w - 1u - k : k;
-            const uint32_t px = __ldg(reinterpret_cast<const uint32_t*>(line + (size_t)ks * step));
+            uint32_t px;                                               // the tap as a BGRA word
+            if constexpr (BPP == 0) px = __ldg(reinterpret_cast<const uint32_t*>(line + (size_t)ks * step));
+            else px = rows_tap_bgra<BPP>(line + (size_t)ks * step);
             const float wt = __ldg(w + (k - l));
             float pb = __ldg(T + (px & 0xffu)), pg = __ldg(T + ((px >> 8) & 0xffu)), pr = __ldg(T + ((px >> 16) & 0xffu)), pa = 0.0f;
             if (am) {
@@ -123,12 +133,8 @@ __global__ void __launch_bounds__(128) hpass_rows_kernel(const JobDev* __restric
         float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
         for (uint32_t k = l; k <= r; ++k) {
             uint32_t px;                                               // the tap as a BGRA word
-            if constexpr (BPP == 3) {
-                const uint8_t* p = src + (size_t)k * 3;
-                px = (uint32_t)__ldg(p + 2) | ((uint32_t)__ldg(p + 1) << 8) | ((uint32_t)__ldg(p) << 16) | 0xff000000u;
-            } else {
-                px = __byte_perm(__ldg(reinterpret_cast<const uint32_t*>(src) + k), 0u, 0x3012);
-            }
+            if constexpr (BPP == 3) px = rows_tap_bgra<3>(src + (size_t)k * 3);
+            else px = __byte_perm(__ldg(reinterpret_cast<const uint32_t*>(src) + k), 0u, 0x3012);   // rows_tap_bgra<4>, indexed as before
             const float wt = __ldg(w + (k - l));
             float pb = __ldg(T + (px & 0xffu)), pg = __ldg(T + ((px >> 8) & 0xffu)), pr = __ldg(T + ((px >> 16) & 0xffu)), pa = 0.0f;
             if (am) {

@@ -10,7 +10,7 @@ from typing import Optional, Sequence
 import numpy as np
 
 from ._lib import (CanvasDesc, ColorDesc, ColorStep, DetectContentDesc, OrientDesc, OrientedResampleDesc, PixelConvertDesc, ResampleDesc, RoundCornersDesc,
-                   RowsResampleDesc, WatermarkDesc, lib)
+                   RowsOrientedResampleDesc, RowsResampleDesc, WatermarkDesc, lib)
 
 
 class Filter(enum.IntEnum):
@@ -492,14 +492,21 @@ def oriented_source_window(window: BitmapWindow, orientation: int, x1: int, y1: 
     """The sub-window of the stored `window` whose orientation by `orientation` is the crop [x1, x2) x [y1, y2) of the oriented frame
     (None when the crop is not inside it): a crop after ApplyOrientation (the crop step of Constrain) rides the same
     Batch.scale_and_render_oriented job.  The preimage of an axis-aligned rectangle under these eight symmetries is one."""
+    r = oriented_source_rect(window.w, window.h, orientation, x1, y1, x2, y2)
+    return None if r is None else window.window(*r)
+
+
+def oriented_source_rect(w: int, h: int, orientation: int, x1: int, y1: int, x2: int, y2: int) -> Optional[tuple]:
+    """oriented_source_window's rectangle (sx1, sy1, sx2, sy2) in a stored w x h frame, or None: for decoder rows, the crop of a
+    Batch.scale_and_render_rows_oriented job is rows[sy1:sy2, sx1:sx2]."""
     t, fx, fy = _ORIENTATION.get(int(orientation), _ORIENTATION[1])
-    ow, oh = (window.h, window.w) if t else (window.w, window.h)
+    ow, oh = (h, w) if t else (w, h)
     if not (0 <= x1 < x2 <= ow and 0 <= y1 < y2 <= oh):
         return None
     ax, ay = ((y1, y2), (x1, x2)) if t else ((x1, x2), (y1, y2))     # the oriented ranges along source x and source y
-    sx1, sx2 = (window.w - ax[1], window.w - ax[0]) if fx else ax
-    sy1, sy2 = (window.h - ay[1], window.h - ay[0]) if fy else ay
-    return window.window(sx1, sy1, sx2, sy2)
+    sx1, sx2 = (w - ax[1], w - ax[0]) if fx else ax
+    sy1, sy2 = (h - ay[1], h - ay[0]) if fy else ay
+    return sx1, sy1, sx2, sy2
 
 
 def apply_orientation(window: BitmapWindow, flag: int, device: int = 0):
@@ -1262,6 +1269,41 @@ class Batch:
         RgbaToBgra, not opaque).  Asynchronous on `stream`; nothing is written when an argument is rejected."""
         descs, keep = self.make_rows_descs(jobs)
         self.enqueue_rows(descs, stream, keep)
+
+    def make_rows_oriented_descs(self, jobs):
+        """jobs: iterable of (rows, canvas BitmapWindow, ScaleAndRenderParams, orientation[, color_matrix[, alpha_meaningful]]); `rows`
+        as make_rows_descs takes them, as the decoder wrote them (not rotated); `orientation` the EXIF flag."""
+        jobs = list(jobs)
+        arr = (RowsOrientedResampleDesc * len(jobs))()
+        keep = []
+        for i, j in enumerate(jobs):
+            if isinstance(j[0], BitmapWindow):
+                raise FlowError(ErrorKind.InvalidArgument, f"oriented rows resample job {i}: a BitmapWindow is already BGRA; resample it "
+                                                           "with scale_and_render_oriented")
+            rows = PixelRows.of(j[0])
+            am = (rows.channels == 4) if len(j) < 6 or j[5] is None else bool(j[5])
+            src = BitmapWindow(rows.ptr, rows.w, rows.h, rows.stride, alpha_meaningful=am, _keep=rows._keep)
+            _fill_desc(arr[i].draw, src, j[1], j[2], j[4] if len(j) > 4 else None, keep)
+            arr[i].format = self._ROWS_FORMAT.get(rows.channels, -1)
+            arr[i].orientation = int(j[3])
+            keep.append(rows._keep)
+        keep.append([j[1]._keep for j in jobs])                         # the bitmaps stay alive until sync() / close()
+        return arr, keep
+
+    def enqueue_rows_oriented(self, descs, stream=None, keep=None) -> None:
+        if keep:
+            self._keep.append(keep)
+        buf = C.create_string_buffer(512)
+        _check(lib().ifb200_batch_enqueue_rows_oriented(self._h, descs, len(descs), self._stream(stream), buf, 512), buf)
+
+    def scale_and_render_rows_oriented(self, jobs, stream=None) -> None:
+        """scale_and_render(orient(to_bgra(rows), orientation), canvas, params) on DEVICE decoder rows without the BGRA frame or the
+        oriented frame being written: jobs: iterable of (rows, canvas, ScaleAndRenderParams, orientation[, color_matrix[,
+        alpha_meaningful]]) as make_rows_oriented_descs takes them -- e.g. nvJPEG's (H, W, 3) RGB tensor and the photo's EXIF flag.  A
+        crop of the oriented frame is a slice of the rows at oriented_source_rect.  Asynchronous on `stream`; nothing is written when
+        an argument is rejected."""
+        descs, keep = self.make_rows_oriented_descs(jobs)
+        self.enqueue_rows_oriented(descs, stream, keep)
 
     def color_matrix(self, dev_ptr: int, w: int, h: int, stride: int, m, stream=None) -> None:
         mm = np.ascontiguousarray(m, np.float32).reshape(25)

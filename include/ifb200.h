@@ -306,6 +306,21 @@ typedef struct ifb200_rows_resample_desc {
     int32_t format;
 } ifb200_rows_resample_desc;
 
+/* One resample of oriented decoder rows: scale_and_render(orient(to_bgra(draw.in, format), orientation), canvas, params), byte for
+ * byte, without the BGRA frame or the oriented frame ever being written -- a phone photo that a GPU decoder wrote as RGB24 rows, with
+ * its EXIF orientation, straight into a thumbnail.
+ *   draw         draw.in / in_w / in_h / in_stride: the rows as the decoder wrote them (not rotated); the resample sees in_w x in_h
+ *                for 1..4 and in_h x in_w for 5..8.  Every other field as in ifb200_batch_enqueue.
+ *   format       as in ifb200_rows_resample_desc, with the same row rules (checked on the stored rows).  Gray8 and GrayAlpha8 rows are
+ *                refused: convert them with ifb200_batch_pixel_convert, then call ifb200_batch_enqueue_oriented.
+ *   orientation  EXIF flag as in ifb200_oriented_resample_desc; values other than 2..8 are the identity.
+ * The arithmetic is that of ifb200_oriented_resample_desc on the BGRA frame to_bgra gives. */
+typedef struct ifb200_rows_oriented_resample_desc {
+    ifb200_resample_desc draw;
+    int32_t format;
+    int32_t orientation;
+} ifb200_rows_oriented_resample_desc;
+
 /* One frame of ifb200_batch_detect_content_many: detect_content (graphics/whitespace.rs:284-331) of the DEVICE BGRA window px
  * (w x h, row pitch `stride` bytes), grayscale Bgra32 when alpha_meaningful != 0 else Bgr32, edges where the Scharr value exceeds
  * `threshold`.  The limits are those of ifb200_batch_detect_content: a non-empty window, w and h below 2^31, threshold below 2^31. */
@@ -344,6 +359,16 @@ int  ifb200_batch_enqueue_oriented(ifb200_batch* b, const ifb200_oriented_resamp
  * written.  ifb200_batch_fused_jobs / ifb200_batch_generic_jobs count these jobs too. */
 int  ifb200_batch_enqueue_rows(ifb200_batch* b, const ifb200_rows_resample_desc* d, size_t n, void* cuda_stream,
                                char* err, size_t err_cap);
+/* n resamples of oriented DEVICE decoder rows (ifb200_rows_oriented_resample_desc), asynchronous on `cuda_stream`, as
+ * ifb200_batch_enqueue.  Neither the BGRA frame nor the oriented frame is written: conversion and orientation both happen in the
+ * resample's source reads.  Down-scales run the streaming ring kernel (RGBA32: the rules of ifb200_batch_enqueue_oriented; RGB24: a
+ * pitch that is a multiple of 16 bytes, the window at any byte and any width); up-scales, 1:1, other windows and
+ * IFB200_OPT_FORCE_GENERIC run the generic pair with an H pass that orients and converts its taps.  Identity jobs run exactly as
+ * ifb200_batch_enqueue_rows runs them.  Every descriptor is checked ("oriented rows resample job i: ...") and every plan built
+ * before anything is enqueued, so an error means nothing is written.  ifb200_batch_fused_jobs / ifb200_batch_generic_jobs count
+ * these jobs too. */
+int  ifb200_batch_enqueue_rows_oriented(ifb200_batch* b, const ifb200_rows_oriented_resample_desc* d, size_t n, void* cuda_stream,
+                                        char* err, size_t err_cap);
 int  ifb200_batch_color_matrix(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride,
                                const float m[25], void* cuda_stream, char* err, size_t err_cap);
 int  ifb200_batch_apply_matte(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride,

@@ -16,7 +16,15 @@ source pixel, two-step 3 or 4 + 4 + 4, floor 4, each + 4 B per output pixel.  Ex
 needs.  The card's name and power limit are read in the same run and printed with the numbers.
 --profile: instead, one torch.profiler run (CUDA activity) of the fused call and of the floor at row (a), printing the CUDA time per
 kernel name: the RGB24 ring kernel against the BGRA ring kernel on the same geometry.
-Usage: python tools/bench_rows.py [--trials 5] [--json out.json] [--profile]"""
+--oriented: the oriented rows resample (Batch.scale_and_render_rows_oriented -> ifb200_batch_enqueue_rows_oriented) instead, same
+method, against the two-step route (Batch.pixel_convert, then Batch.scale_and_render_oriented), the rows floor (the rows resample of
+rows that are already oriented) and the BGRA floor (the plain resample of oriented BGRA frames).  Rows:
+  (o1) 256 x 4032x3024 RGB24, flag 6 -> 384x512;  (o2) the same, flag 8
+  (o3) 64 x 3840x2160 RGB24, flag 3 -> 512x288
+  (o4) 64 x 3840x2160 RGBA32 with cut-out alpha, flag 6 -> 288x512
+  (o5) 16 x 640x480 RGB24, flag 6 -> 960x1280 (an up-scale: the generic pair)
+With --profile: the RGB24 transposed ring kernel (row o1) against the stored RGB24 ring kernel on the same oriented geometry.
+Usage: python tools/bench_rows.py [--trials 5] [--json out.json] [--profile] [--oriented]"""
 import argparse, json, os, subprocess, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -131,11 +139,95 @@ def profile(batch, stream, n=64, iw=3840, ih=2160):
     torch.cuda.empty_cache()
 
 
+def orient_t(a, flag):
+    """the (n, h, w, c) frames oriented by the EXIF flag, contiguous (the closed form of include/ifb200.h)"""
+    t, fx, fy = {2: (0, 1, 0), 3: (0, 1, 1), 4: (0, 0, 1), 5: (1, 0, 0), 6: (1, 0, 1), 7: (1, 1, 1), 8: (1, 1, 0)}.get(flag, (0, 0, 0))
+    dims = [d for d, f in ((1, fy), (2, fx)) if f]
+    b = a.flip(dims) if dims else a
+    return (b.transpose(1, 2) if t else b).contiguous()
+
+
+def oriented_setup(batch, n, iw, ih, bpp, flag, ow, oh, cutout=False):
+    dev = torch.device("cuda:0")
+    buf, rows = frames(n, iw, ih, bpp, None, cutout)
+    rows_o = orient_t(rows, flag)                                                 # the rows floor's input: rows already oriented
+    scratch = torch.empty((n, ih, iw, 4), dtype=torch.uint8, device=dev)          # the two-step route's BGRA frames
+    outs = [torch.zeros((n, oh, ow, 4), dtype=torch.uint8, device=dev) for _ in range(4)]
+    p = ifb.ScaleAndRenderParams(w=ow, h=oh)
+    am = bpp == 4
+    win = lambda a, i: ifb.BitmapWindow.from_torch(a[i], alpha_meaningful=am)
+    op = ifb.pixel_op_for(bpp)
+    batch.pixel_convert([op(ifb.PixelRows.from_torch(rows[i]), win(scratch, i)) for i in range(n)], torch.cuda.current_stream().cuda_stream)
+    scratch_o = orient_t(scratch, flag)                                           # the BGRA floor's input
+    d = dict(fused_d=batch.make_rows_oriented_descs([(rows[i], win(outs[0], i), p, flag) for i in range(n)]),
+             oriented_d=batch.make_oriented_descs([(win(scratch, i), win(outs[1], i), p, flag) for i in range(n)]),
+             rows_floor_d=batch.make_rows_descs([(rows_o[i], win(outs[2], i), p) for i in range(n)]),
+             floor_d=batch.make_descs([(win(scratch_o, i), win(outs[3], i), p) for i in range(n)]))
+    convert_jobs = [op(ifb.PixelRows.from_torch(rows[i]), win(scratch, i)) for i in range(n)]
+    return dict(buf=buf, rows=rows, rows_o=rows_o, scratch=scratch, scratch_o=scratch_o, outs=outs, convert_jobs=convert_jobs,
+                **{k: v[0] for k, v in d.items()})
+
+
+def oriented_row(batch, stream, name, n, iw, ih, bpp, flag, ow, oh, trials, cutout=False):
+    s = oriented_setup(batch, n, iw, ih, bpp, flag, ow, oh, cutout)
+    counts = lambda: (batch.fused_jobs, batch.generic_jobs, batch.tile_jobs)
+    c0 = counts()
+    batch.enqueue_rows_oriented(s["fused_d"], stream)
+    torch.cuda.synchronize()
+    path = {k: int(v) for k, v in zip(("ring", "generic", "tile"), np.subtract(counts(), c0)) if v}
+    fused, fts = timed(lambda: batch.enqueue_rows_oriented(s["fused_d"], stream), trials)
+
+    def two_step():
+        batch.pixel_convert(s["convert_jobs"], stream)
+        batch.enqueue_oriented(s["oriented_d"], stream)
+    two, tts = timed(two_step, trials)
+    rows_floor, _ = timed(lambda: batch.enqueue_rows(s["rows_floor_d"], stream), trials)
+    floor, _ = timed(lambda: batch.enqueue(s["floor_d"], stream), trials)
+    torch.cuda.synchronize()
+    outs = s["outs"]
+    assert all(torch.equal(outs[0], o) for o in outs[1:]), (name, "routes differ")
+    r = dict(row=name, frames=n, size=f"{iw}x{ih}", fmt="RGBA32" if bpp == 4 else "RGB24", flag=flag, out=f"{ow}x{oh}", path=path,
+             fused_ms=round(fused, 3), two_step_ms=round(two, 3), rows_floor_ms=round(rows_floor, 3), bgra_floor_ms=round(floor, 3),
+             fused_over_rows_floor=round(fused / rows_floor, 3), fused_over_two_step=round(fused / two, 3),
+             two_step_scratch_bytes=int(s["scratch"].numel()), bit_exact=True,
+             fused_trials=[round(x, 3) for x in fts], two_step_trials=[round(x, 3) for x in tts])
+    print(json.dumps(r), flush=True)
+    del s, outs
+    batch._keep.clear()
+    torch.cuda.empty_cache()
+    return r
+
+
+def oriented_profile(batch, stream, n=256, iw=4032, ih=3024, flag=6):
+    """kernel time of the fused call (RGB24 rows, transposed reads) and of the rows floor (the stored RGB24 form on the same oriented
+    geometry), per kernel name"""
+    from torch.profiler import ProfilerActivity, profile as tprofile
+    s = oriented_setup(batch, n, iw, ih, 3, flag, 384, 512)
+    for name, d, fn in (("fused", s["fused_d"], batch.enqueue_rows_oriented), ("rows_floor", s["rows_floor_d"], batch.enqueue_rows)):
+        for _ in range(2):
+            fn(d, stream)
+        torch.cuda.synchronize()
+        with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(5):
+                fn(d, stream)
+            torch.cuda.synchronize()
+        ks = {}
+        for e in prof.events():
+            if e.device_type.name == "CUDA":
+                ks.setdefault(e.name, []).append(e.device_time_total if hasattr(e, "device_time_total") else e.cuda_time_total)
+        for k, v in ks.items():
+            print(json.dumps(dict(route=name, kernel=k[:100], launches=len(v), median_us=round(float(np.median(v)), 1))), flush=True)
+    del s
+    batch._keep.clear()
+    torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--trials", type=int, default=5)
     ap.add_argument("--json", default=None)
     ap.add_argument("--profile", action="store_true")
+    ap.add_argument("--oriented", action="store_true")
     a = ap.parse_args()
     torch.cuda.set_device(0)
     info = card()
@@ -143,7 +235,16 @@ def main():
     batch = ifb.Batch(0)
     stream = torch.cuda.current_stream().cuda_stream
     if a.profile:
-        profile(batch, stream)
+        (oriented_profile if a.oriented else profile)(batch, stream)
+        return
+    if a.oriented:
+        rows = [oriented_row(batch, stream, "o1", 256, 4032, 3024, 3, 6, 384, 512, a.trials),
+                oriented_row(batch, stream, "o2", 256, 4032, 3024, 3, 8, 384, 512, a.trials),
+                oriented_row(batch, stream, "o3", 64, 3840, 2160, 3, 3, 512, 288, a.trials),
+                oriented_row(batch, stream, "o4", 64, 3840, 2160, 4, 6, 288, 512, a.trials, cutout=True),
+                oriented_row(batch, stream, "o5", 16, 640, 480, 3, 6, 960, 1280, a.trials)]
+        if a.json:
+            json.dump({"card": info, "rows": rows}, open(a.json, "w"), indent=1)
         return
     rows = [row(batch, stream, "a", 64, 3840, 2160, 3, 512, 288, a.trials),
             row(batch, stream, "b", 256, 4032, 3024, 3, 512, 384, a.trials),
