@@ -23,7 +23,7 @@ SYMBOLS = [
     "ifb200_block_scale_u8", "ifb200_batch_block_scale", "ifb200_round_corners_bgra8", "ifb200_batch_round_corners",
     "ifb200_batch_canvas", "ifb200_batch_orient", "ifb200_batch_color_chain", "ifb200_batch_watermark",
     "ifb200_batch_pixel_convert", "ifb200_batch_enqueue_oriented", "ifb200_batch_enqueue_rows", "ifb200_batch_detect_content_many",
-    "ifb200_batch_enqueue_rows_oriented",
+    "ifb200_batch_enqueue_rows_oriented", "ifb200_batch_transform_to_srgb", "ifb200_source_profile_plan",
 ]
 
 
@@ -105,6 +105,23 @@ class PixelConvertDesc(C.Structure):
         ("op", C.c_int32), ("src", C.c_void_p), ("src_stride", C.c_uint32), ("dst", C.c_void_p), ("dst_stride", C.c_uint32),
         ("w", C.c_uint32), ("h", C.c_uint32), ("opaque", C.c_int32),
     ]
+
+
+class SourceProfileDesc(C.Structure):
+    """struct ifb200_source_profile"""
+    _fields_ = [("kind", C.c_int32), ("icc", C.c_void_p), ("icc_len", C.c_size_t), ("gamma", C.c_double), ("chrm", C.c_double * 8),
+                ("cicp", C.c_uint8 * 4)]
+
+
+class ProfilePlan(C.Structure):
+    """struct ifb200_profile_plan"""
+    _fields_ = [("kind", C.c_int32), ("trc", (C.c_float * 256) * 3), ("m", (C.c_float * 3) * 3), ("gray", C.c_uint8 * 256)]
+
+
+class ToSrgbDesc(C.Structure):
+    """struct ifb200_to_srgb_desc"""
+    _fields_ = [("format", C.c_int32), ("src", C.c_void_p), ("src_stride", C.c_uint32), ("dst", C.c_void_p), ("dst_stride", C.c_uint32),
+                ("w", C.c_uint32), ("h", C.c_uint32), ("profile", C.c_void_p)]
 
 
 class DetectContentDesc(C.Structure):
@@ -218,6 +235,10 @@ def lib() -> C.CDLL:
     L.ifb200_batch_watermark.restype = C.c_int
     L.ifb200_batch_pixel_convert.argtypes = [C.c_void_p, C.POINTER(PixelConvertDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_pixel_convert.restype = C.c_int
+    L.ifb200_batch_transform_to_srgb.argtypes = [C.c_void_p, C.POINTER(ToSrgbDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
+    L.ifb200_batch_transform_to_srgb.restype = C.c_int
+    L.ifb200_source_profile_plan.argtypes = [C.POINTER(SourceProfileDesc), C.POINTER(ProfilePlan), C.c_char_p, C.c_size_t]
+    L.ifb200_source_profile_plan.restype = C.c_int
     L.ifb200_batch_ring_status.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_ring_status.restype = C.c_int
     _lib = L

@@ -1476,6 +1476,26 @@ void pixel_convert_locked(ifb200_batch* b, const ifb200_pixel_convert_desc* d, s
     b->launches++;
 }
 
+// The profile transforms of ifb200_batch_transform_to_srgb (ifb_profile.h): every descriptor is checked and every distinct profile
+// planned before anything is enqueued, then all jobs run in ONE launch (none when no job writes a pixel).  The upload is the items,
+// their first CTAs and plan indices, and the distinct plans: O(jobs + profiles).
+void transform_to_srgb_locked(ifb200_batch* b, const ifb200_to_srgb_desc* d, size_t n, cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    ifb::PfWork wk;
+    int code = 0;
+    const std::string why = ifb::transform_to_srgb_prepare(d, n, wk, &code);
+    if (!why.empty()) IFB_THROW(code, "%s", why.c_str());
+    if (wk.pc.items.empty()) return;
+    if (wk.pc.ctas() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
+    DeviceScope dev_scope_(b->device);
+    WorkUpload up(b, st, {part(wk.pc.items), part(wk.pc.first), part(wk.plan_of), part(wk.plans)});
+    transform_to_srgb_kernel<<<(unsigned)wk.pc.ctas(), ifb::kPcThreads, 0, st>>>(up.at<const ifb::PcItem>(0), up.at<const uint32_t>(1),
+                                                                                 up.at<const uint32_t>(2), up.at<const ifb200_profile_plan>(3),
+                                                                                 b->lut16k.p, (uint32_t)wk.pc.items.size());
+    CUDA_OK(cudaGetLastError());
+    b->launches++;
+}
+
 // The colour chains of ifb200_batch_color_chain (ifb_color.h): every descriptor is checked before anything is planned or enqueued.
 // The plan (jobs, prefix sums, segments, tables, matrices) goes up in one copy, O(jobs + steps); then ONE launch, or three when some
 // job white-balances (histograms into zeroed counters, byte maps into the jobs' kClWb tables, apply); none when no job writes a pixel.
@@ -2029,6 +2049,20 @@ int ifb200_batch_orient(ifb200_batch* b, const ifb200_orient_desc* d, size_t n, 
 
 int ifb200_batch_pixel_convert(ifb200_batch* b, const ifb200_pixel_convert_desc* d, size_t n, void* stream, char* err, size_t cap) {
     return with_batch(b, stream, err, cap, [&](cudaStream_t st) { pixel_convert_locked(b, d, n, st); });
+}
+
+int ifb200_batch_transform_to_srgb(ifb200_batch* b, const ifb200_to_srgb_desc* d, size_t n, void* stream, char* err, size_t cap) {
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { transform_to_srgb_locked(b, d, n, st); });
+}
+
+int ifb200_source_profile_plan(const ifb200_source_profile* p, ifb200_profile_plan* plan, char* why, size_t cap) {
+    return guarded(why, cap, [&] {
+        if (!p) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null profile pointer");
+        ifb200_profile_plan local;
+        std::string reason;
+        const int code = ifb::profile_plan(*p, plan ? plan : &local, &reason);
+        if (code) IFB_THROW(code, "%s", reason.c_str());
+    });
 }
 
 int ifb200_batch_color_chain(ifb200_batch* b, const ifb200_color_desc* d, size_t n, void* stream, char* err, size_t cap) {

@@ -9,8 +9,8 @@ from typing import Optional, Sequence
 
 import numpy as np
 
-from ._lib import (CanvasDesc, ColorDesc, ColorStep, DetectContentDesc, OrientDesc, OrientedResampleDesc, PixelConvertDesc, ResampleDesc, RoundCornersDesc,
-                   RowsOrientedResampleDesc, RowsResampleDesc, WatermarkDesc, lib)
+from ._lib import (CanvasDesc, ColorDesc, ColorStep, DetectContentDesc, OrientDesc, OrientedResampleDesc, PixelConvertDesc, ProfilePlan, ResampleDesc,
+                   RoundCornersDesc, RowsOrientedResampleDesc, RowsResampleDesc, SourceProfileDesc, ToSrgbDesc, WatermarkDesc, lib)
 
 
 class Filter(enum.IntEnum):
@@ -1142,6 +1142,81 @@ def pixel_op_for(channels: int, to_bgra: bool = True):
     return ops[channels]
 
 
+# ---------------------------------------------------------------- colour profiles to sRGB (Batch.transform_to_srgb)
+@dataclass(frozen=True)
+class SourceProfile:
+    """A decoder's colour profile (codecs/source_profile.rs:7-41, CMYK excluded), as include/ifb200.h ifb200_source_profile.  Build it
+    with srgb(), icc(bytes), icc_gray(bytes), gamma_primaries(gamma, wx, wy, rx, ry, gx, gy, bx, by) or cicp(cp, tc, mc, full); which
+    PNG chunk wins stays with the decoder."""
+    SRGB, ICC, ICC_GRAY, GAMMA_PRIMARIES, CICP = range(5)
+    kind: int
+    icc_bytes: bytes = b""
+    gamma: float = 0.0
+    chrm: tuple = (0.0,) * 8
+    cicp_codes: tuple = (0, 0, 0, 0)
+
+    @staticmethod
+    def srgb() -> "SourceProfile":
+        return SourceProfile(SourceProfile.SRGB)
+
+    @staticmethod
+    def icc(data: bytes) -> "SourceProfile":
+        return SourceProfile(SourceProfile.ICC, bytes(data))
+
+    @staticmethod
+    def icc_gray(data: bytes) -> "SourceProfile":
+        return SourceProfile(SourceProfile.ICC_GRAY, bytes(data))
+
+    @staticmethod
+    def gamma_primaries(gamma: float, *chrm: float) -> "SourceProfile":
+        """gamma: the PNG gAMA value (the encoding gamma, e.g. 0.45455); chrm: white, red, green, blue x, y (cHRM)"""
+        if len(chrm) != 8:
+            raise FlowError(ErrorKind.InvalidArgument, f"gamma_primaries takes 8 chromaticities (white, red, green, blue x, y), not {len(chrm)}")
+        return SourceProfile(SourceProfile.GAMMA_PRIMARIES, gamma=float(gamma), chrm=tuple(float(v) for v in chrm))
+
+    @staticmethod
+    def cicp(cp: int, tc: int, mc: int = 0, full: bool = True) -> "SourceProfile":
+        return SourceProfile(SourceProfile.CICP, cicp_codes=(int(cp), int(tc), int(mc), int(bool(full))))
+
+    def _desc(self) -> SourceProfileDesc:
+        """the C struct; it points into self.icc_bytes, which must outlive the call"""
+        d = SourceProfileDesc()
+        d.kind = self.kind
+        if self.icc_bytes:
+            d.icc = C.cast(C.c_char_p(self.icc_bytes), C.c_void_p)
+            d.icc_len = len(self.icc_bytes)
+        d.gamma = self.gamma
+        for i, v in enumerate(self.chrm):
+            d.chrm[i] = v
+        for i, v in enumerate(self.cicp_codes):
+            d.cicp[i] = v
+        return d
+
+
+@dataclass
+class ProfilePlanResult:
+    """What the library plans for a profile (ifb200_profile_plan): kind 0 identity, 1 matrix (trc (3, 256) f32 tables, m (3, 3) f32),
+    2 gray (trc[0] and the 256-byte map)."""
+    IDENTITY, MATRIX, GRAY = range(3)
+    kind: int
+    trc: np.ndarray
+    m: np.ndarray
+    gray: np.ndarray
+
+
+def source_profile_plan(profile: SourceProfile) -> ProfilePlanResult:
+    """The host plan of `profile` (no device needed).  Raises FlowError MethodNotImplemented for a profile the GPU does not run (LUT,
+    Lab PCS, CMYK, PQ / HLG, ...: keep that frame on the CPU CMS) and InvalidArgument for a malformed one, with the reason."""
+    d, plan = profile._desc(), ProfilePlan()
+    buf = C.create_string_buffer(512)
+    _check(lib().ifb200_source_profile_plan(C.byref(d), C.byref(plan), buf, 512), buf)
+    return ProfilePlanResult(plan.kind, np.ctypeslib.as_array(plan.trc).copy(), np.ctypeslib.as_array(plan.m).copy(),
+                             np.ctypeslib.as_array(plan.gray).copy())
+
+
+PROFILE_SRC_BGRA = 16                                              # include/ifb200.h IFB200_PROFILE_SRC_BGRA
+
+
 def device_count() -> int:
     return lib().ifb200_device_count()
 
@@ -1470,6 +1545,43 @@ class Batch:
             out.append(dst)
         self._keep.append([(s._keep, d._keep) for s, d in zip(srcs, dsts)])
         return out
+
+    def transform_to_srgb(self, jobs, stream=None) -> list:
+        """transform_to_srgb(to_bgra(src), profile) (codecs/cms.rs:68 under the moxcms backend) on DEVICE frames, all jobs in one kernel
+        launch (none when no job writes a pixel), asynchronous on `stream`.  jobs: iterable of (src, dst, profile): src a BGRA
+        BitmapWindow or decoder rows (PixelRows.of(), 1..4 channels: Gray8, GrayAlpha8, RGB24, RGBA32), dst a BGRA BitmapWindow of the
+        same size or None for in place (a BitmapWindow src only), profile a SourceProfile.  Every profile is planned before anything is
+        enqueued: an unsupported one raises MethodNotImplemented, a malformed one InvalidArgument, and nothing is written.  Returns the
+        destinations; one written from rows gets alpha_meaningful as pixel_convert sets it."""
+        jobs = list(jobs)
+        a = (ToSrgbDesc * len(jobs))()
+        profs, keep, outs = [], [], []
+        for d, (src, dst, profile) in zip(a, jobs):
+            if not isinstance(profile, SourceProfile):
+                raise FlowError(ErrorKind.InvalidArgument, f"not a SourceProfile: {profile!r}")
+            bgra = isinstance(src, BitmapWindow)
+            if dst is None:
+                if not bgra:
+                    raise FlowError(ErrorKind.InvalidArgument, "in place needs a BGRA BitmapWindow source")
+                dst = src
+            s, t = PixelRows.of(src), PixelRows.of(dst)
+            if t.channels != 4 or (s.w, s.h) != (t.w, t.h):
+                raise FlowError(ErrorKind.InvalidArgument, f"transform_to_srgb writes a BGRA frame the size of its source, not "
+                                                           f"{t.w}x{t.h}x{t.channels} from {s.w}x{s.h}x{s.channels}")
+            d.format = PROFILE_SRC_BGRA if bgra else pixel_op_for(s.channels).OP
+            d.src, d.src_stride, d.dst, d.dst_stride, d.w, d.h = s.ptr, s.stride, t.ptr, t.stride, s.w, s.h
+            pd = profile._desc()
+            profs.append((pd, profile))
+            d.profile = C.cast(C.byref(pd), C.c_void_p)
+            keep.append((s._keep, t._keep))
+            outs.append(dst)
+        buf = C.create_string_buffer(512)
+        _check(lib().ifb200_batch_transform_to_srgb(self._h, a, len(jobs), self._stream(stream), buf, 512), buf)
+        for (src, _, _), dst in zip(jobs, outs):
+            if isinstance(dst, BitmapWindow) and dst is not src:
+                dst.alpha_meaningful = src.alpha_meaningful if isinstance(src, BitmapWindow) else PixelRows.of(src).channels in (2, 4)
+        self._keep.append(keep)
+        return outs
 
     def to_bgra(self, rows, opaque: bool = False, stream=None) -> "BitmapWindow":
         """One call from decoder rows -- an (H, W, C) uint8 CUDA tensor, C in 1..4, or PixelRows -- to a new BGRA BitmapWindow on the

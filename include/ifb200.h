@@ -293,6 +293,57 @@ typedef struct ifb200_pixel_convert_desc {
     int32_t        opaque;                  /* != 0: alpha = 255 in a 4-byte output */
 } ifb200_pixel_convert_desc;
 
+/* A decoder's colour profile (the reference's SourceProfile, codecs/source_profile.rs:7-41, CMYK excluded) and the transform of a
+ * frame to sRGB under it: transform_to_srgb(to_bgra(src, format), profile) as codecs/moxcms_transform.rs runs it with
+ * lut_transform_opts() (relative colorimetric), for the profiles whose transform is a matrix-shaper.  Kinds:
+ *   SRGB             the identity (is_srgb()): in place nothing is written; from rows the output is ifb200_batch_pixel_convert's.
+ *   ICC              icc / icc_len: an ICC profile (v2 or v4) with colour space 'RGB ', PCS 'XYZ ', rXYZ / gXYZ / bXYZ and rTRC / gTRC /
+ *                    bTRC tags.  A TRC is 'curv' (0 entries: identity; 1: u8Fixed8 gamma; more: a table interpolated linearly) or
+ *                    'para' (function types 0-4, ICC.1:2010 §10.18; a power of a negative base is 0).
+ *   ICC_GRAY         icc / icc_len: colour space 'GRAY' with a kTRC tag.  The gray value is the B byte of to_bgra(src); B, G and R all
+ *                    get the transformed value, alpha is kept (moxcms_transform.rs:356-376).
+ *   GAMMA_PRIMARIES  gamma: the PNG gAMA value (the encoding gamma); the TRC is x^f32(1 / gamma).  chrm: white, red, green, blue x,y.
+ *   CICP             cicp = {colour primaries, transfer characteristics, matrix coefficients, full range}: primaries any code of
+ *                    H.273 table 2 (1, 4-12, 22); transfer 1/6/14/15 (BT.709), 4 (gamma 2.2), 5 (gamma 2.8), 7 (SMPTE 240M),
+ *                    8 (linear) or 13 (sRGB); matrix coefficients 0; full range.  Primaries 1 with transfer 13 is SRGB.
+ * The plan, in float64 rounded once to f32: T_c[v] = f32(clip01(trc_c(v / 255))), v = 0..255, and M = f32(S^-1 C), where C is the
+ * source colorants (rXYZ gXYZ bXYZ as stored -- chad / wtpt not applied -- or, for GAMMA_PRIMARIES and CICP, the chromaticities'
+ * colorants Bradford-adapted to D50) and S the sRGB colorants (BT.709 primaries, D65) Bradford-adapted to D50 (0.9642, 1, 0.8249).
+ * Per pixel, in f32 without contraction: o_c = (M[c][0] T_r[r] + M[c][1] T_g[g]) + M[c][2] T_b[b], and the byte is the resample's
+ * linear-to-sRGB table at trunc(clamp(o_c * 16383, 0, 16383)) (the clamp is the clip to [0, 1], NaN -> 0).  A gray plan is one byte
+ * map, gray[v] = that encode of T[v].  Alpha passes unchanged (RGB24 and Gray8 sources: 255, as to_bgra gives).
+ * Refused with IFB200_ERR_NOT_IMPLEMENTED (keep such a frame on the CPU CMS): A2B0-2, B2A0-2, D2B0-3 or B2D0-3 tags; mft1, mft2,
+ * 'mAB ' or 'mBA ' tag types; a Lab PCS; CMYK or any colour space but RGB and GRAY; CICP transfer PQ (16), HLG (18) or any code not
+ * listed; unknown CICP primaries; matrix coefficients other than 0; narrow range.  Refused with IFB200_ERR_INVALID_ARGUMENT: a
+ * truncated or malformed profile (every offset and size is checked against icc_len; nothing outside the buffer is read), a colour
+ * space that does not match the kind (an RGB profile as ICC_GRAY and the reverse), a gamma or chromaticity that gives no matrix. */
+enum ifb200_profile_kind { IFB200_PROFILE_SRGB = 0, IFB200_PROFILE_ICC = 1, IFB200_PROFILE_ICC_GRAY = 2,
+                           IFB200_PROFILE_GAMMA_PRIMARIES = 3, IFB200_PROFILE_CICP = 4 };
+typedef struct ifb200_source_profile {
+    int32_t        kind;                    /* enum ifb200_profile_kind */
+    const uint8_t* icc; size_t icc_len;     /* HOST bytes for the ICC kinds; read before the call returns */
+    double         gamma;                   /* GAMMA_PRIMARIES: the gAMA value */
+    double         chrm[8];                 /* GAMMA_PRIMARIES: white x, y, red x, y, green x, y, blue x, y */
+    uint8_t        cicp[4];                 /* CICP: primaries, transfer, matrix coefficients, full range (0 / 1) */
+} ifb200_source_profile;
+/* What a profile plans to (ifb200_source_profile_plan). */
+enum ifb200_plan_kind { IFB200_PLAN_IDENTITY = 0, IFB200_PLAN_MATRIX = 1, IFB200_PLAN_GRAY = 2 };
+typedef struct ifb200_profile_plan {
+    int32_t kind;                           /* enum ifb200_plan_kind */
+    float   trc[3][256];                    /* MATRIX: T_r, T_g, T_b; GRAY: T in trc[0] */
+    float   m[3][3];                        /* MATRIX: M[output r, g, b][input r, g, b] */
+    uint8_t gray[256];                      /* GRAY: the byte map */
+} ifb200_profile_plan;
+/* The source of a transform: a BGRA window, or decoder rows of one of the four ifb200_pixel_op *_TO_BGRA ops. */
+#define IFB200_PROFILE_SRC_BGRA 16
+typedef struct ifb200_to_srgb_desc {
+    int32_t        format;                  /* IFB200_PROFILE_SRC_BGRA or IFB200_PIXEL_{RGB24,RGBA,GRAY,GRAY_ALPHA}_TO_BGRA */
+    const uint8_t* src; uint32_t src_stride;   /* w x h source rows; BGRA with src == dst and the same stride: in place */
+    uint8_t*       dst; uint32_t dst_stride;   /* w x h BGRA destination: 4-byte aligned pointer and stride */
+    uint32_t       w, h;
+    const ifb200_source_profile* profile;   /* HOST pointer, read before the call returns */
+} ifb200_to_srgb_desc;
+
 /* One resample of decoder rows: scale_and_render(to_bgra(draw.in, format), canvas, params), byte for byte, without the BGRA frame
  * ever being written -- the decode -> DrawImageExact chain of a frame a GPU decoder wrote as interleaved rows (nvJPEG's RGB24, the
  * PNG and WebP decoders' RGBA32).  to_bgra is the ifb200_pixel_convert_desc op `format` with opaque = 0.
@@ -444,6 +495,18 @@ int  ifb200_batch_watermark(ifb200_batch* b, const ifb200_watermark_desc* d, siz
  * enqueued, so an error means nothing is written.  There is no host-buffer variant: on host rows the decoders' own loop is cheaper than
  * the trip over PCIe. */
 int  ifb200_batch_pixel_convert(ifb200_batch* b, const ifb200_pixel_convert_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
+/* Colour profiles to sRGB (ifb200_to_srgb_desc, ifb200_source_profile) on n DEVICE windows in ONE kernel launch, none when no job
+ * writes a pixel (SRGB jobs in place, zero-area jobs); asynchronous on `cuda_stream`.  Each destination byte is written once and
+ * nothing outside the two windows is read.  Every descriptor is checked and every profile planned before anything is enqueued, so an
+ * error ("transform to srgb job i: <why>", with the profile's status) means nothing is written; jobs of zero area are skipped
+ * unchecked.  The row rules are ifb200_batch_pixel_convert's; overlap other than exact in-place BGRA is refused.  Identical profile
+ * bytes (or parameters) within one call are planned once.  No job may write what another job of the call reads or writes (not
+ * checked).  There is no host-buffer variant. */
+int  ifb200_batch_transform_to_srgb(ifb200_batch* b, const ifb200_to_srgb_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
+/* Host only, no device needed: IFB200_OK when the GPU runs this profile, IFB200_ERR_NOT_IMPLEMENTED (use the CPU CMS) or
+ * IFB200_ERR_INVALID_ARGUMENT, with the reason in `why`.  When `plan` is not NULL and the status is OK, also the planned tables and
+ * matrix. */
+int  ifb200_source_profile_plan(const ifb200_source_profile* p, ifb200_profile_plan* plan, char* why, size_t why_cap);
 int  ifb200_batch_sync(ifb200_batch* b, char* err, size_t err_cap);
 void ifb200_batch_destroy(ifb200_batch* b);
 /* knobs / introspection (benchmarks, tests) */
