@@ -788,12 +788,14 @@ const HvTmap& tmap_for(ifb200_batch* b, const ifb200_resample_desc& d, uint32_t*
     const cuuint64_t strides[1] = {(cuuint64_t)d.in_stride};
     const cuuint32_t box[2] = {bytes ? (transposed ? 128u : 64u) : transposed ? 32u : 16u, transposed ? 16u : 32u};
     const cuuint32_t estr[2] = {1u, 1u};
-    // L2 promotion: how much of a line a 64-byte box row pulls into L2 (IFB200_DEBUG_L2_PROMOTION = 0 / 64 / 128 / 256 for experiments)
-    static const CUtensorMapL2promotion promo = [] {
-        const char* e = getenv("IFB200_DEBUG_L2_PROMOTION");
-        const int v = e ? atoi(e) : 256;
-        return v == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : v == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : v == 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
-    }();
+    // L2 promotion: how much of a line a box row pulls into L2 (IFB200_DEBUG_L2_PROMOTION = 0 / 64 / 128 / 256 for experiments).
+    // The 64-byte rows of the stored-frame boxes take 128 bytes: the row and the next box's.  With 256 (four boxes' worth) the
+    // 4K -> 512 bench line took 19.2 ms, with 128 17.5 ms, with 64 or none 22.7 ms (DESIGN.md section 5.1).  The transposed
+    // forms' 128-byte rows keep 256.
+    static const int promo_env = [] { const char* e = getenv("IFB200_DEBUG_L2_PROMOTION"); return e ? atoi(e) : -1; }();
+    const int promo_bytes = promo_env >= 0 ? promo_env : transposed ? 256 : 128;
+    const CUtensorMapL2promotion promo = promo_bytes == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : promo_bytes == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B
+                                       : promo_bytes == 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
     const CUresult r = b->tmap_encode(&tm, bytes ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                       transposed ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_64B, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) IFB_THROW(IFB200_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) for a %ux%u bitmap, pitch %u", (int)r, d.in_w, d.in_h, d.in_stride);

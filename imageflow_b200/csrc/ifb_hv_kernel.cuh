@@ -67,6 +67,26 @@ enum : int { HV_SRC_BGRA = 0, HV_SRC_RGBA = 1, HV_SRC_RGB24 = 2 };
 #ifndef IFB_HV_MAXCOLS4
 #define IFB_HV_MAXCOLS4 64             // widest strip of the ring-depth-4 variants (V accumulators: 12 or 16 registers per 16 columns)
 #endif
+#ifndef IFB_HV_STAGES
+#define IFB_HV_STAGES 2                // ring slots per warp (A/B builds: with more, fewer warps fit; DESIGN.md section 5.1)
+#endif
+#ifndef IFB_HV_WARPS3
+#define IFB_HV_WARPS3 16               // warps per CTA with three channels
+#endif
+#ifndef IFB_HV_WARPS4
+#define IFB_HV_WARPS4 12               // and with four
+#endif
+// Probe builds (A/B measurements only, never the product; their outputs are wrong on purpose):
+//   IFB_HV_PROBE_MEM   the TMA stream alone: same boxes, waits and refill points; the H and V arithmetic replaced by one dependent
+//                      use of each chunk's bytes, one word stored per work item
+//   IFB_HV_PROBE_MATH  the arithmetic alone: H pass, V pass and store over boxes fetched once per work item (one per ring slot),
+//                      then read again and again with no refill and no wait
+#ifndef IFB_HV_PROBE_MEM
+#define IFB_HV_PROBE_MEM 0
+#endif
+#ifndef IFB_HV_PROBE_MATH
+#define IFB_HV_PROBE_MATH 0
+#endif
 template <int AV, int CH> struct HvCfg {
     static_assert(AV == 4 || AV == 6, "ring depth");
     static constexpr int kAvp = AV == 4 ? 4 : 8;                      // floats per weight record
@@ -76,9 +96,9 @@ template <int AV, int CH> struct HvCfg {
     static constexpr int kMaxCols = AV == 4 ? IFB_HV_MAXCOLS4 : (CH == 3 ? 50 : 40);   // widest strip (output columns)
     static constexpr int kNG = kMaxCols / kCG + 1;                    // column groups per strip (V accumulators: 2 * CH registers per group); groups end on
                                                                       // chunk-pair boundaries and are not always full, hence one more than the columns need
-    static constexpr int kWarps = CH == 3 ? 16 : 12;
+    static constexpr int kWarps = CH == 3 ? IFB_HV_WARPS3 : IFB_HV_WARPS4;
     static constexpr int kThreads = kWarps * 32;
-    static constexpr int kStages = 2;
+    static constexpr int kStages = IFB_HV_STAGES;                     // boxes in the ring: up to kStages - 1 in flight while one is read
     static constexpr int kBoxBytes = 32 * 64;                         // one box: 32 rows x 16 pixels
     static constexpr int kStageBytes = kBoxBytes;
     static constexpr int kRingBytes = kStages * kStageBytes;
@@ -366,6 +386,7 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
         hv::mbar_init_fence();
     }
     uint32_t par = 0;                                                      // bit s: parity the next wait on stage s expects
+    auto next_slot = [](const int s_) { return S == 2 ? s_ ^ 1 : s_ + 1 == S ? 0 : s_ + 1; };   // ring slots are used in turn
 
     const uint32_t lut_lane = lut + (uint32_t)lane * 4u;
     const uint32_t lane4 = ((uint32_t)lane * 4u) | ((lut >> 16) << 8);     // PRMT operand: byte 0 = lane*4, bytes 1..2 = window bits 16..31
@@ -476,11 +497,11 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
                         else hv::tma_load_box(stb + (uint32_t)is_s * C::kStageBytes, tm, xoff + l0 + (int)zero_dep, s0, bar);
                     }
                 }
-                --tma_left; is_s ^= 1;
+                --tma_left; is_s = next_slot(is_s);
                 tma_x += kBoxX;
                 if (tma_x == x_end) { tma_x = x_origin; tma_y += 32; }
             };
-            static_assert(S == 2, "the slot bookkeeping below toggles between two slots");
+            static_assert(S >= 2, "one slot is read while the next is filled");
             // orientation of the job: which axis of the stream / of the lanes runs backwards through the stored frame (issue() reads
             // the flags itself: declared ahead of it, these change the instruction schedule of the stored-frame form)
             const bool rev_s = ORI == HV_ORI_FLIP ? (flags & JF_FLIP_X) != 0u : ORI == HV_ORI_TRANSPOSE ? (flags & JF_FLIP_Y) != 0u : false;
@@ -534,8 +555,17 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
                 }
             };
 
-            if (tma_left > 0) issue(0u);
+            // boxes are fetched in order into slots 0, 1, .., S - 1, 0, ..: S - 1 here, one more at the start of every row block, and
+            // one whenever a stage (not the last of its row block) has been read, into the slot just read -- S - 1 boxes ahead
+            if constexpr (IFB_HV_PROBE_MATH) {                            // probe: every slot filled once, then only read
+                const int nfill = min(S, tma_left);
+                for (int i = 0; i < nfill; ++i) issue(0u);
+                for (int i = 0; i < nfill; ++i) { hv::mbar_wait(mb + 8u * (uint32_t)i, (par >> i) & 1u); par ^= 1u << i; }
+            } else {
+                for (int i = 0; i < S - 1 && tma_left > 0; ++i) issue(0u);
+            }
             int cs_s = 0;                                                  // ring slot of the stage being consumed
+            uint32_t probe_sink = 0;                                       // IFB_HV_PROBE_MEM: what the chunks' bytes add up to
 
             float2 accV[NG][CH];                                           // this lane's slot pair of column cl of every group
 #pragma unroll
@@ -565,9 +595,11 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
                 uint32_t wcur = lutw;                                      // H weight records of the current chunk pair
 
                 // ---- first stage of the row block
-                if (tma_left > 0) issue(0u);
-                hv::mbar_wait(mb + 8u * (uint32_t)cs_s, (par >> cs_s) & 1u);
-                par ^= 1u << cs_s;
+                if constexpr (!IFB_HV_PROBE_MATH) {
+                    if (tma_left > 0) issue(0u);
+                    hv::mbar_wait(mb + 8u * (uint32_t)cs_s, (par >> cs_s) & 1u);
+                    par ^= 1u << cs_s;
+                }
                 uint32_t sbase = stb + (uint32_t)cs_s * C::kStageBytes + (ORI == HV_ORI_NONE ? (uint32_t)lane * 64u : 0u);
                 uint4 rawA = chunk(sbase, 0u), rawB;             // the sixteen bytes of this lane's row in the pair's first / second chunk
                 uint32_t hd_next = (uint32_t)hv::ldg(hdone + lane);
@@ -633,12 +665,19 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
                     // made to depend on the loaded bytes, so that it cannot overtake the load).
                     rawB = chunk(sbase, ((pc & 1u) << 1) | 1u);
                     if ((pc & 1u) && more) {
-                        cs_s ^= 1;
-                        // (transposed and RGB24: the chunk is four loads, and the refill waits for all of them; RGB24's .x and .w depend on all four)
-                        if (tma_left > 0) issue(hv::zero_after(ORI == HV_ORI_TRANSPOSE ? rawB.x ^ rawB.y ^ rawB.z ^ rawB.w : SRC == HV_SRC_RGB24 ? rawB.x ^ rawB.w : rawB.x, pl.zero));
-                        hv::mbar_wait(mb + 8u * (uint32_t)cs_s, (par >> cs_s) & 1u);
-                        par ^= 1u << cs_s;
+                        cs_s = next_slot(cs_s);
+                        if constexpr (!IFB_HV_PROBE_MATH) {
+                            // (transposed and RGB24: the chunk is four loads, and the refill waits for all of them; RGB24's .x and .w depend on all four)
+                            if (tma_left > 0) issue(hv::zero_after(ORI == HV_ORI_TRANSPOSE ? rawB.x ^ rawB.y ^ rawB.z ^ rawB.w : SRC == HV_SRC_RGB24 ? rawB.x ^ rawB.w : rawB.x, pl.zero));
+                            hv::mbar_wait(mb + 8u * (uint32_t)cs_s, (par >> cs_s) & 1u);
+                            par ^= 1u << cs_s;
+                        }
                         sbase = stb + (uint32_t)cs_s * C::kStageBytes + (ORI == HV_ORI_NONE ? (uint32_t)lane * 64u : 0u);
+                    }
+                    if constexpr (IFB_HV_PROBE_MEM) {                      // probe: the pair's bytes, used once; no H or V pass
+                        probe_sink += rawA.x ^ rawA.y ^ rawA.z ^ rawA.w ^ rawB.x ^ rawB.y ^ rawB.z ^ rawB.w;
+                        rawA = chunk(sbase, ((pc + 1u) & 1u) << 1);
+                        continue;
                     }
                     // behind the pair's seventh column: the next pair's first chunk (chunk 2 pc + 2; behind the last pair of the row block: bytes nobody uses)
 #define IFB_HV_RELOAD rawA = chunk(sbase, ((pc + 1u) & 1u) << 1);
@@ -805,10 +844,14 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
                     }
                   }
                 }
-                cs_s ^= 1;
+                cs_s = next_slot(cs_s);
                 // every group of the row block has seen the same rows: commit the vertical position
                 Yc += (int)vtot;
                 vslot = (vslot + vtot) % (uint32_t)AV;
+            }
+            if constexpr (IFB_HV_PROBE_MEM) {
+                const uint32_t v = hv::warp_sum(probe_sink);
+                if (lane == 0) *reinterpret_cast<uint32_t*>(job.out + (size_t)sX0 * 4 + (size_t)bY0 * out_stride) = v;
             }
         }
     }
