@@ -81,11 +81,17 @@ enum : int { HV_SRC_BGRA = 0, HV_SRC_RGBA = 1, HV_SRC_RGB24 = 2 };
 //                      use of each chunk's bytes, one word stored per work item
 //   IFB_HV_PROBE_MATH  the arithmetic alone: H pass, V pass and store over boxes fetched once per work item (one per ring slot),
 //                      then read again and again with no refill and no wait
+//   IFB_HV_PROBE_NOPARK  (with IFB_HV_PROBE_MATH) every chunk with one completion runs as the plain form: the arithmetic side
+//                      without the cost of parking a column (the column is counted and its place in the exchange buffer
+//                      advanced; no slot is picked, its values are never stored or cleared)
 #ifndef IFB_HV_PROBE_MEM
 #define IFB_HV_PROBE_MEM 0
 #endif
 #ifndef IFB_HV_PROBE_MATH
 #define IFB_HV_PROBE_MATH 0
+#endif
+#ifndef IFB_HV_PROBE_NOPARK
+#define IFB_HV_PROBE_NOPARK 0
 #endif
 template <int AV, int CH> struct HvCfg {
     static_assert(AV == 4 || AV == 6, "ring depth");
@@ -684,12 +690,15 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
                     // A chunk (four source columns) exists in six compiled forms, picked by tests whose operands are known long before
                     // they are needed: no completion (plain straight-line code: about half of the chunks of a 7.5 : 1 down-scale); exactly
                     // one completion and no column that completes twice -- one form per ring slot of the completing column, with a
-                    // predicated "park and clear" of that slot behind every column (no branch inside, no look-up of the slot); and
-                    // the general form with a test behind every column.
+                    // predicated "park and clear" of that slot behind every column (no branch inside, no look-up of the slot) and one
+                    // unconditional advance of xw behind the chunk; and the general form with a test behind every column.  The plain
+                    // form is tested first: it is the most frequent, and then takes one branch.  More compiled forms (one per slot and
+                    // column, or per slot and half chunk) cut the instructions of a one-completion chunk further but made the kernel
+                    // slower (DESIGN.md section 5.1).
 #define IFB_HV_ACC(S_, C_) (((S_) & 1) ? accH[C_][((S_) % AV) / 2].y : accH[C_][((S_) % AV) / 2].x)
 #define IFB_HV_PF(S_, BIT_, M_) { \
-        if (CH == 3) hv::flush3_if<BIT_, kXCol>(xw, IFB_HV_ACC(S_, 0), IFB_HV_ACC(S_, 1), IFB_HV_ACC(S_, 2), M_); \
-        else hv::flush4_if<BIT_, kXCol>(xw, IFB_HV_ACC(S_, 0), IFB_HV_ACC(S_, 1), IFB_HV_ACC(S_, 2), IFB_HV_ACC(S_, CH - 1), M_); }
+        if (CH == 3) hv::flush3_if<BIT_, 0u>(xw, IFB_HV_ACC(S_, 0), IFB_HV_ACC(S_, 1), IFB_HV_ACC(S_, 2), M_); \
+        else hv::flush4_if<BIT_, 0u>(xw, IFB_HV_ACC(S_, 0), IFB_HV_ACC(S_, 1), IFB_HV_ACC(S_, 2), IFB_HV_ACC(S_, CH - 1), M_); }
 #define IFB_HV_NONE
 #define IFB_HV_STEPS_A(F0_, F1_, F2_, F3_) { \
         wload(W1, wcur + kRec); conv(P1, rawA.y); mac(P0, W0); F0_ \
@@ -703,19 +712,21 @@ hv_ring_kernel(const JobDev* __restrict__ jobs, const HvTmap* __restrict__ tmaps
         wload(W0, wnext); conv(P0, rawA.x); mac(P1, W1); F3_ }
 #define IFB_HV_CHUNK(STEPS_, SH_) { \
         const uint32_t m4_ = (hm >> (SH_)) & 15u; \
-        if (IFB_HV_NOFAST || ((((hm2 >> (SH_)) & 15u) | (m4_ & (m4_ - 1u))) != 0u)) { \
-            STEPS_(IFB_HV_FLUSH((SH_) + 0), IFB_HV_FLUSH((SH_) + 1), IFB_HV_FLUSH((SH_) + 2), IFB_HV_FLUSH((SH_) + 3)) \
-        } else if (m4_ == 0u) { \
+        if (!IFB_HV_NOFAST && m4_ == 0u) { \
             STEPS_(IFB_HV_NONE, IFB_HV_NONE, IFB_HV_NONE, IFB_HV_NONE) \
+        } else if (IFB_HV_NOFAST || ((((hm2 >> (SH_)) & 15u) | (m4_ & (m4_ - 1u))) != 0u)) { \
+            STEPS_(IFB_HV_FLUSH((SH_) + 0), IFB_HV_FLUSH((SH_) + 1), IFB_HV_FLUSH((SH_) + 2), IFB_HV_FLUSH((SH_) + 3)) \
         } else { \
-            if (hslot < 2u) { \
+            if (IFB_HV_PROBE_NOPARK) { \
+                STEPS_(IFB_HV_NONE, IFB_HV_NONE, IFB_HV_NONE, IFB_HV_NONE) \
+            } else if (hslot < 2u) { \
                 if (hslot == 0u) IFB_HV_FORM(STEPS_, 0) else IFB_HV_FORM(STEPS_, 1) \
             } else if (AV == 4 || hslot < 4u) { \
                 if (hslot == 2u) IFB_HV_FORM(STEPS_, 2) else IFB_HV_FORM(STEPS_, 3) \
             } else { \
                 if (hslot == 4u) IFB_HV_FORM(STEPS_, 4) else IFB_HV_FORM(STEPS_, 5) \
             } \
-            ++colbuf; hslot = hslot + 1u == (uint32_t)AV ? 0u : hslot + 1u; \
+            xw += kXCol; ++colbuf; hslot = hslot + 1u == (uint32_t)AV ? 0u : hslot + 1u; \
         } }
 #define IFB_HV_FORM(STEPS_, K_) STEPS_(IFB_HV_PF((K_) % AV, 1u, m4_), IFB_HV_PF((K_) % AV, 2u, m4_), IFB_HV_PF((K_) % AV, 4u, m4_), IFB_HV_PF((K_) % AV, 8u, m4_))
                     IFB_HV_CHUNK(IFB_HV_STEPS_A, 0)

@@ -1,9 +1,11 @@
 #!/usr/bin/env python3
 """Split the ring kernel's time on the bench line into its memory side and its arithmetic side.
 
-Builds libifb200.so three times into OUT (each from a private copy of the sources, so builds run side by side and nothing in the
+Builds libifb200.so four times into OUT (each from a private copy of the sources, so builds run side by side and nothing in the
 tree is written): `product` (the library as shipped), `mem` (-DIFB_HV_PROBE_MEM=1: the TMA stream with its waits and refills,
-no H or V arithmetic) and `math` (-DIFB_HV_PROBE_MATH=1: the H pass, V pass and store over boxes fetched once per work item).
+no H or V arithmetic), `math` (-DIFB_HV_PROBE_MATH=1: the H pass, V pass and store over boxes fetched once per work item) and
+`nopark` (`math` with -DIFB_HV_PROBE_NOPARK=1: every chunk with one completion runs as the plain form, so that its time against
+`math` is what parking the completed columns costs).
 Then runs bench.py on each through IFB200_LIB, the libraries alternating, ROUNDS times, and prints the kernel time (CUDA events)
 of every run and the median / min / max per library, with the card's name, power limit and SM clock.
 
@@ -26,7 +28,7 @@ import sys
 import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PROBES = {"product": "", "mem": "-DIFB_HV_PROBE_MEM=1", "math": "-DIFB_HV_PROBE_MATH=1"}
+PROBES = {"product": "", "mem": "-DIFB_HV_PROBE_MEM=1", "math": "-DIFB_HV_PROBE_MATH=1", "nopark": "-DIFB_HV_PROBE_MATH=1 -DIFB_HV_PROBE_NOPARK=1"}
 
 
 def build_one(tag: str, flags: str, out: str) -> str:
@@ -108,7 +110,7 @@ def main() -> None:
         for wl in workloads:
             for t in variants:
                 wl_name = wl or "c2_4k_to_512_robidoux"
-                r = run_bench(libs[t], wl_name, a.batch, a.steps, a.warmup, check=t not in ("mem", "math"))
+                r = run_bench(libs[t], wl_name, a.batch, a.steps, a.warmup, check=t not in PROBES or t == "product")
                 r.update(tag=t, workload=wl_name, round=rnd)
                 res["runs"].append(r)
                 print(json.dumps(r), flush=True)
