@@ -26,7 +26,8 @@ Host-side mirror of the reference seam (paths relative to the imageflow checkout
       RGB24 / RGBA32 conversion whose only consumer is the resample folded into its reads (Batch.scale_and_render_rows), also
       together with an ApplyOrientation (Batch.scale_and_render_rows_oriented; a crop in between via oriented_source_rect)
   codecs/cms.rs:68, moxcms_transform.rs  transform_to_srgb of a frame with a matrix/TRC ICC, gray ICC, gAMA+cHRM or CICP profile, from a
-      BGRA frame in place or from decoder rows, batched (Batch.transform_to_srgb, SourceProfile; source_profile_plan routes a frame)
+      BGRA frame in place or from decoder rows, batched (Batch.transform_to_srgb, SourceProfile; source_profile_plan routes a frame);
+      folded into the resample's source reads with the orientation (Batch.scale_and_render_profiled)
   c_components/lib/codecs_jpeg_idct_fast.c  flow_scale_spatial[_srgb]_NxN (decode-time JPEG block scalers)
 All arithmetic runs in hand-written sm_90a kernels inside libifb200.so (include/ifb200.h);
 this package only marshals arguments.  Nothing here imports the CPU oracle.
@@ -43,7 +44,7 @@ from .graphics import (Batch, apply_matte, BitmapCompositing, BitmapWindow, Erro
                        process_constraint, watermark_layout, riapi_watermark_placement, PixelRows, RgbToBgra, RgbaToBgra, GrayToBgra,
                        GrayAlphaToBgra, BgraToRgb, pixel_op_for, CropWhitespace, riapi_trim_steps, crop_whitespace_bounds, SourceProfile,
                        ProfilePlanResult, source_profile_plan)
-from ._lib import LIB_PATH, ResampleDesc, RowsOrientedResampleDesc, RowsResampleDesc, lib
+from ._lib import LIB_PATH, ProfiledResampleDesc, ResampleDesc, RowsOrientedResampleDesc, RowsResampleDesc, lib
 
 __all__ = [
     "Batch", "apply_matte", "BitmapCompositing", "BitmapWindow", "ErrorKind", "Filter", "FlowError", "ScaleAndRenderParams",
@@ -57,6 +58,6 @@ __all__ = [
     "riapi_color_steps", "Watermark", "WatermarkConstraintBox", "WatermarkConstraintMode", "ConstraintGravity", "WatermarkDraw",
     "process_constraint", "watermark_layout", "riapi_watermark_placement", "PixelRows", "RgbToBgra", "RgbaToBgra", "GrayToBgra",
     "GrayAlphaToBgra", "BgraToRgb", "pixel_op_for", "CropWhitespace", "riapi_trim_steps", "crop_whitespace_bounds", "SourceProfile",
-    "ProfilePlanResult", "source_profile_plan", "LIB_PATH", "ResampleDesc", "RowsOrientedResampleDesc",
+    "ProfilePlanResult", "source_profile_plan", "LIB_PATH", "ProfiledResampleDesc", "ResampleDesc", "RowsOrientedResampleDesc",
     "RowsResampleDesc", "lib",
 ]

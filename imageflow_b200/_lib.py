@@ -24,6 +24,7 @@ SYMBOLS = [
     "ifb200_batch_canvas", "ifb200_batch_orient", "ifb200_batch_color_chain", "ifb200_batch_watermark",
     "ifb200_batch_pixel_convert", "ifb200_batch_enqueue_oriented", "ifb200_batch_enqueue_rows", "ifb200_batch_detect_content_many",
     "ifb200_batch_enqueue_rows_oriented", "ifb200_batch_transform_to_srgb", "ifb200_source_profile_plan",
+    "ifb200_batch_enqueue_profiled",
 ]
 
 
@@ -122,6 +123,11 @@ class ToSrgbDesc(C.Structure):
     """struct ifb200_to_srgb_desc"""
     _fields_ = [("format", C.c_int32), ("src", C.c_void_p), ("src_stride", C.c_uint32), ("dst", C.c_void_p), ("dst_stride", C.c_uint32),
                 ("w", C.c_uint32), ("h", C.c_uint32), ("profile", C.c_void_p)]
+
+
+class ProfiledResampleDesc(C.Structure):
+    """struct ifb200_profiled_resample_desc"""
+    _fields_ = [("draw", ResampleDesc), ("format", C.c_int32), ("orientation", C.c_int32), ("profile", C.c_void_p)]
 
 
 class DetectContentDesc(C.Structure):
@@ -237,6 +243,8 @@ def lib() -> C.CDLL:
     L.ifb200_batch_pixel_convert.restype = C.c_int
     L.ifb200_batch_transform_to_srgb.argtypes = [C.c_void_p, C.POINTER(ToSrgbDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_transform_to_srgb.restype = C.c_int
+    L.ifb200_batch_enqueue_profiled.argtypes = [C.c_void_p, C.POINTER(ProfiledResampleDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
+    L.ifb200_batch_enqueue_profiled.restype = C.c_int
     L.ifb200_source_profile_plan.argtypes = [C.POINTER(SourceProfileDesc), C.POINTER(ProfilePlan), C.c_char_p, C.c_size_t]
     L.ifb200_source_profile_plan.restype = C.c_int
     L.ifb200_batch_ring_status.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t]

@@ -415,11 +415,18 @@ using HvFn = void (*)(const JobDev*, const HvTmap*, Tables, HvPlanDev, uint32_t,
 // fn[ORI][EPI] reads BGRA frames, rows[SRC - 1][EPI] the rows of ifb200_batch_enqueue_rows (HV_SRC_RGBA, HV_SRC_RGB24),
 // rows_ori[SRC - 1][ORI - 1][EPI] those of ifb200_batch_enqueue_rows_oriented; EPI: general, simple + linear, simple + sRGB.  A null
 // entry is a form that is not compiled (its jobs take the generic pair).
-struct HvEntry { int av, ch; HvFn fn[3][3]; int threads, warps, max_cols, ng; uint32_t (*smem)(uint32_t); HvFn rows[2][3]; HvFn rows_ori[2][2][3]; };
-HvFn hv_form(const HvEntry* e, int ori, int src, int epi) {
+// prof[PROF - 1][ORI][SRC][EPI - 1]: the forms of ifb200_batch_enqueue_profiled (PF_MATRIX, PF_GRAY), with pthreads / pwarps /
+// psmem[PROF - 1] in place of threads / warps / smem.  They exist for the simple store epilogues only: a profiled job with the general
+// one takes the generic pair.
+struct HvEntry {
+    int av, ch; HvFn fn[3][3]; int threads, warps, max_cols, ng; uint32_t (*smem)(uint32_t); HvFn rows[2][3]; HvFn rows_ori[2][2][3];
+    HvFn prof[2][3][3][2]; int pthreads, pwarps; uint32_t (*psmem[2])(uint32_t);
+};
+HvFn hv_form(const HvEntry* e, int ori, int src, int epi, int prof = PF_IDENTITY) {
+    if (prof != PF_IDENTITY) return epi == 0 ? nullptr : e->prof[prof - 1][ori][src][epi - 1];
     return src == HV_SRC_BGRA ? e->fn[ori][epi] : ori == HV_ORI_NONE ? e->rows[src - 1][epi] : e->rows_ori[src - 1][ori - 1][epi];
 }
-template <int AV, int CH> uint32_t hv_smem_bytes(uint32_t sb_low16) { return hv_total_bytes<AV, CH>(sb_low16); }
+template <int AV, int CH, int PROF = PF_IDENTITY> uint32_t hv_smem_bytes(uint32_t sb_low16) { return hv_total_bytes<AV, CH, PROF>(sb_low16); }
 #define IFB_HV_EPI(AV_, CH_, O_) {hv_ring_kernel<AV_, CH_, 0, O_>, hv_ring_kernel<AV_, CH_, 1, O_>, hv_ring_kernel<AV_, CH_, 2, O_>}
 // The RGB24 form with the general store epilogue at ring depth 6 and three channels spills (one register over the 128 of 16 warps):
 // it is not compiled, and its jobs take the generic pair (enqueue_locked)
@@ -435,9 +442,15 @@ template <> constexpr HvFn kRowsOriented<6, 3, 1, HV_ORI_FLIP, HV_SRC_RGB24> = n
 #define IFB_HV_RO(AV_, CH_, O_, S_) {kRowsOriented<AV_, CH_, 0, O_, S_>, kRowsOriented<AV_, CH_, 1, O_, S_>, kRowsOriented<AV_, CH_, 2, O_, S_>}
 #define IFB_HV_ROWS_ORI(AV_, CH_) {{IFB_HV_RO(AV_, CH_, HV_ORI_FLIP, HV_SRC_RGBA), IFB_HV_RO(AV_, CH_, HV_ORI_TRANSPOSE, HV_SRC_RGBA)}, \
                                    {IFB_HV_RO(AV_, CH_, HV_ORI_FLIP, HV_SRC_RGB24), IFB_HV_RO(AV_, CH_, HV_ORI_TRANSPOSE, HV_SRC_RGB24)}}
+#define IFB_HV_PF_E(AV_, CH_, O_, S_, P_) {hv_ring_profiled_kernel<AV_, CH_, 1, O_, S_, P_>, hv_ring_profiled_kernel<AV_, CH_, 2, O_, S_, P_>}
+#define IFB_HV_PF_S(AV_, CH_, O_, P_) {IFB_HV_PF_E(AV_, CH_, O_, HV_SRC_BGRA, P_), IFB_HV_PF_E(AV_, CH_, O_, HV_SRC_RGBA, P_), IFB_HV_PF_E(AV_, CH_, O_, HV_SRC_RGB24, P_)}
+#define IFB_HV_PF(AV_, CH_, P_) {IFB_HV_PF_S(AV_, CH_, HV_ORI_NONE, P_), IFB_HV_PF_S(AV_, CH_, HV_ORI_FLIP, P_), IFB_HV_PF_S(AV_, CH_, HV_ORI_TRANSPOSE, P_)}
 #define IFB_HV(AV_, CH_) {AV_, CH_, {IFB_HV_EPI(AV_, CH_, HV_ORI_NONE), IFB_HV_EPI(AV_, CH_, HV_ORI_FLIP), IFB_HV_EPI(AV_, CH_, HV_ORI_TRANSPOSE)}, \
                           HvCfg<AV_, CH_>::kThreads, HvCfg<AV_, CH_>::kWarps, HvCfg<AV_, CH_>::kMaxCols, HvCfg<AV_, CH_>::kNG, hv_smem_bytes<AV_, CH_>, \
-                          IFB_HV_SRC(AV_, CH_), IFB_HV_ROWS_ORI(AV_, CH_)}
+                          IFB_HV_SRC(AV_, CH_), IFB_HV_ROWS_ORI(AV_, CH_), {IFB_HV_PF(AV_, CH_, PF_MATRIX), IFB_HV_PF(AV_, CH_, PF_GRAY)}, \
+                          HvCfg<AV_, CH_, PF_MATRIX>::kThreads, HvCfg<AV_, CH_, PF_MATRIX>::kWarps, \
+                          {hv_smem_bytes<AV_, CH_, PF_MATRIX>, hv_smem_bytes<AV_, CH_, PF_GRAY>}}
+static_assert(HvCfg<4, 3, PF_MATRIX>::kWarps == HvCfg<4, 3, PF_GRAY>::kWarps && HvCfg<4, 4, PF_MATRIX>::kWarps == HvCfg<4, 4, PF_GRAY>::kWarps, "one warp count per profiled variant");
 const HvEntry kHv[] = {IFB_HV(4, 3), IFB_HV(4, 4), IFB_HV(6, 3), IFB_HV(6, 4)};
 const HvEntry* find_hv(int av, int ch) {
     for (const auto& e : kHv) if (e.av == av && e.ch == ch) return &e;
@@ -826,8 +839,10 @@ uint32_t ori_flips(int flag) {
 // src != nullptr (enqueue_rows_locked): descs[i].in holds rows of format src[i] (HV_SRC_RGBA / HV_SRC_RGB24), checked by the
 // caller; these jobs take the ring kernel's row forms or the generic pair with hpass_rows_kernel (there is no tile-kernel form).
 // Both (enqueue_rows_oriented_locked): the ring kernel's oriented row forms or the generic pair with hpass_oriented_kernel<TR, BPP>.
+// plan != nullptr (enqueue_profiled_locked): plan[i] is job i's profile plan, null for an identity plan; jobs with a plan take the
+// ring kernel's profiled forms (one launch per plan) or the generic pair with hpass_oriented_kernel<TR, BPP, PROF> (flag 1 included).
 void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n, cudaStream_t st, const int32_t* ori = nullptr,
-                    const int32_t* src = nullptr) {
+                    const int32_t* src = nullptr, const ifb200_profile_plan* const* plan = nullptr) {
     if (!descs && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
     if (n == 0) return;
     Tick tk_all(b->prof.enqueue);
@@ -838,7 +853,8 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
     { Tick tk(b->prof.plans); b->prebuild_plans(descs, n); }
     // group jobs by (plan, kernel class)
     // kind: 0 generic pair, 1 ring kernel, 3 tile kernel (`variant` = its compile-time case)
-    struct Group { Plan* plan; int ch; int kind; bool simple; int variant; int ori; int src; std::vector<size_t> idx; int cols_key = 0; };
+    struct Group { Plan* plan; int ch; int kind; bool simple; int variant; int ori; int src; const ifb200_profile_plan* prof; std::vector<size_t> idx; int cols_key = 0;
+                   int pk() const { return prof ? prof->kind : PF_IDENTITY; } };
     std::vector<Group> groups;
     for (size_t i = 0; i < n; ++i) {
         Plan* pp; { Tick tk(b->prof.plans); pp = &b->plan_for(descs[i]); }
@@ -861,19 +877,22 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
             if (sf == HV_SRC_RGB24) ring = p.hv_ok && b->ring_ok && !b->force_generic && (d.in_stride % 16 == 0);
             if (upscale) ring = false;
         }
+        const ifb200_profile_plan* const jp = plan ? plan[i] : nullptr;
+        const int pk = jp ? jp->kind : PF_IDENTITY;
+        if (pk != PF_IDENTITY && upscale) ring = false;                // profiled up-scales and 1:1: the generic pair
         const bool simple = d.compose == IFB200_REPLACE_SELF && !d.color_matrix;   // store epilogue without composite / matrix code
-        if (ring && sf != HV_SRC_BGRA && !hv_form(find_hv(p.av, ch), oc, sf, simple ? (d.linear ? 1 : 2) : 0)) ring = false;   // a form not compiled
+        if (ring && (sf != HV_SRC_BGRA || pk != PF_IDENTITY) && !hv_form(find_hv(p.av, ch), oc, sf, simple ? (d.linear ? 1 : 2) : 0, pk)) ring = false;   // a form not compiled
         if (ring && !(p.tile_ok && upscale) && !hv_host_ready(p, hv_cols(p.av, ch, b->strip_cols))) ring = false;   // windows wider than the weight table
         // the ring kernel streams every source row once and wins whenever rows outnumber outputs (down-scales);
         // for up-scales / 1:1 the tile kernel does less work per source pixel
-        const bool prefer_tile = oc == HV_ORI_NONE && sf == HV_SRC_BGRA && p.tile_ok && !b->force_generic && (!ring || upscale);
+        const bool prefer_tile = oc == HV_ORI_NONE && sf == HV_SRC_BGRA && pk == PF_IDENTITY && p.tile_ok && !b->force_generic && (!ring || upscale);
         const int kind = prefer_tile ? 3 : (ring ? 1 : 0);
         // the ring kernel keeps ONE transfer table per CTA: jobs of different working spaces go to different launches
         const int variant = kind == 3 ? ((d.linear ? 1 : 0) | ((ch == 4 ? d.compose : 0) << 1) | (d.color_matrix ? 8 : 0)) : kind == 1 ? (d.linear ? 1 : 0) : 0;
         Group* g = nullptr;
         for (auto& gg : groups)
-            if (gg.plan == &p && gg.ch == ch && gg.kind == kind && gg.simple == simple && gg.variant == variant && gg.ori == oc && gg.src == sf) { g = &gg; break; }
-        if (!g) { groups.push_back(Group{&p, ch, kind, simple, variant, oc, sf, {}}); g = &groups.back(); }
+            if (gg.plan == &p && gg.ch == ch && gg.kind == kind && gg.simple == simple && gg.variant == variant && gg.ori == oc && gg.src == sf && gg.prof == jp) { g = &gg; break; }
+        if (!g) { groups.push_back(Group{&p, ch, kind, simple, variant, oc, sf, jp, {}}); g = &groups.back(); }
         g->idx.push_back(i);
     }
     // Strip width of every ring group: the widest (least halo) that still gives every warp of the device an item; a launch for one
@@ -882,7 +901,7 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
         if (g.kind != 1) continue;
         Plan& p = *g.plan;
         const HvEntry* he = find_hv(p.av, g.ch);
-        const size_t warps_all = (size_t)b->sm_count * he->warps;
+        const size_t warps_all = (size_t)b->sm_count * (g.prof ? he->pwarps : he->warps);
         const size_t max_nb = std::max<uint32_t>(1u, p.out_h / 8u);
         g.cols_key = hv_cols(p.av, g.ch, b->strip_cols);
         if (b->min_items == 0)
@@ -922,18 +941,19 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
     auto take = [&](size_t nbytes) { const size_t o = (bytes + 127) / 128 * 128; bytes = o + nbytes; return o; };
     for (size_t gi = 0; gi < groups.size(); ++gi) {
         Group& g = groups[gi];
-        lay[gi].jobs = take(g.idx.size() * sizeof(JobDev));
+        lay[gi].jobs = take(g.idx.size() * sizeof(JobDev) + (g.prof ? sizeof(ProfDev) : 0));   // a plan follows the job array
         if (g.kind == 1) {
             Plan& p = *g.plan;
             const HvEntry* he = find_hv(p.av, g.ch);
             const HvTables& ht = *p.by_cols.at(g.cols_key);
             const size_t jxs = g.idx.size() * (size_t)ht.n_strips;
-            const int warps_all = b->sm_count * he->warps;
+            const int warps = g.prof ? he->pwarps : he->warps;
+            const int warps_all = b->sm_count * warps;
             const int nb = hv_pick_bands(p, jxs, warps_all, b->min_items);
             lay[gi].bv = hv_bands(p, nb);
             lay[gi].nb = (int)lay[gi].bv.size();
             const size_t items = jxs * nb;
-            lay[gi].grid = (int)std::min<size_t>((size_t)b->sm_count, (items + he->warps - 1) / he->warps);
+            lay[gi].grid = (int)std::min<size_t>((size_t)b->sm_count, (items + warps - 1) / warps);
             lay[gi].tmaps = take(g.idx.size() * sizeof(HvTmap));
             lay[gi].bands = take(lay[gi].bv.size() * sizeof(HvBandDev));
             lay[gi].counters = take((size_t)ht.n_strips * sizeof(uint32_t));
@@ -955,6 +975,10 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
                 uint32_t xoff = 0; ht[pos] = tmap_for(b, stored, &xoff, g.ori == HV_ORI_TRANSPOSE, g.src == HV_SRC_RGB24); hj[pos].in_xoff = xoff;
             }
             ++pos;
+        }
+        if (g.prof) {
+            ProfDev* pd = reinterpret_cast<ProfDev*>(hj + pos);
+            memcpy(pd->trc, g.prof->trc, sizeof pd->trc); memcpy(pd->m, g.prof->m, sizeof pd->m); memcpy(pd->gray, g.prof->gray, sizeof pd->gray);
         }
         if (g.kind == 1) {
             memcpy(hbuf + lay[gi].bands, lay[gi].bv.data(), lay[gi].bv.size() * sizeof(HvBandDev));
@@ -1029,13 +1053,13 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
             pl.vw = ht.blob.at<float>(ht.o_vw); pl.vdone = ht.blob.at<uint8_t>(ht.o_vdone);
             pl.hw_stride = ht.hw_stride;
             const int epi = g.simple ? ((g.variant & 1) ? 1 : 2) : 0;       // the ring kernel's launches are per working space (variant bit 0 = linear)
-            HvFn fn = hv_form(he, g.ori, g.src, epi);
-            const size_t smem = he->smem(b->smem_base_low16);
+            HvFn fn = hv_form(he, g.ori, g.src, epi, g.pk());
+            const size_t smem = g.prof ? he->psmem[g.pk() - 1](b->smem_base_low16) : he->smem(b->smem_base_low16);
             if (!b->hv_attr_set.count((const void*)fn)) {
                 CUDA_OK(cudaFuncSetAttribute((const void*)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
                 b->hv_attr_set.insert((const void*)fn);
             }
-            fn<<<(unsigned)lay[gi].grid, he->threads, smem, st>>>(jobs, reinterpret_cast<const HvTmap*>(dbuf + lay[gi].tmaps), b->tables, pl, (uint32_t)nj,
+            fn<<<(unsigned)lay[gi].grid, g.prof ? he->pthreads : he->threads, smem, st>>>(jobs, reinterpret_cast<const HvTmap*>(dbuf + lay[gi].tmaps), b->tables, pl, (uint32_t)nj,
                                                                   reinterpret_cast<uint32_t*>(dbuf + lay[gi].counters));
             CUDA_OK(cudaGetLastError());
             b->launches++;
@@ -1051,21 +1075,25 @@ void enqueue_locked(ifb200_batch* b, const ifb200_resample_desc* descs, size_t n
             AsyncFree inter_guard{inter, st};
             for (size_t off = 0; off < nj; off += chunk) {
                 const size_t cnt = std::min(chunk, nj - off);
-                if (g.ori == HV_ORI_NONE && g.src != HV_SRC_BGRA) {
+                if (g.ori == HV_ORI_NONE && g.src != HV_SRC_BGRA && !g.prof) {
                     dim3 gh((p.out_w + 127) / 128, std::min<uint32_t>(p.in_h, 65535u), (unsigned)cnt);
                     if (g.src == HV_SRC_RGB24) hpass_rows_kernel<3><<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_h, p.out_w, inter);
                     else hpass_rows_kernel<4><<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_h, p.out_w, inter);
-                } else if (g.ori == HV_ORI_NONE) {
+                } else if (g.ori == HV_ORI_NONE && !g.prof) {
                     dim3 gh((p.out_w + 127) / 128, std::min<uint32_t>(p.in_h, 65535u), (unsigned)cnt);
                     hpass_generic_kernel<<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_h, p.out_w, inter);
                 } else {
                     // flips: threads along output columns; transposes: threads along oriented rows = along a source row
                     const bool tr = g.ori == HV_ORI_TRANSPOSE;
                     dim3 gh(((tr ? p.in_h : p.out_w) + 127) / 128, std::min<uint32_t>(tr ? p.out_w : p.in_h, 65535u), (unsigned)cnt);
-                    using HFn = void (*)(const JobDev*, Tables, AxisDev, uint32_t, uint32_t, uint32_t, float4*);
-                    static const HFn kOriented[2][3] = {{hpass_oriented_kernel<false>, hpass_oriented_kernel<false, 4>, hpass_oriented_kernel<false, 3>},
-                                                        {hpass_oriented_kernel<true>, hpass_oriented_kernel<true, 4>, hpass_oriented_kernel<true, 3>}};
-                    kOriented[tr][g.src]<<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_w, p.in_h, p.out_w, inter);
+                    // (profiled jobs: also flag 1, the form without flips; the plan follows the group's job array)
+                    using HFn = void (*)(const JobDev*, Tables, AxisDev, uint32_t, uint32_t, uint32_t, float4*, const ProfDev*);
+#define IFB_HO(P_) {{hpass_oriented_kernel<false, 0, P_>, hpass_oriented_kernel<false, 4, P_>, hpass_oriented_kernel<false, 3, P_>}, \
+                    {hpass_oriented_kernel<true, 0, P_>, hpass_oriented_kernel<true, 4, P_>, hpass_oriented_kernel<true, 3, P_>}}
+                    static const HFn kOriented[3][2][3] = {IFB_HO(PF_IDENTITY), IFB_HO(PF_MATRIX), IFB_HO(PF_GRAY)};
+#undef IFB_HO
+                    const ProfDev* pd = g.prof ? reinterpret_cast<const ProfDev*>(jobs + nj) : nullptr;
+                    kOriented[g.pk()][tr][g.src]<<<gh, 128, 0, st>>>(jobs + off, b->tables, p.dh.view(*p.axes), p.in_w, p.in_h, p.out_w, inter, pd);
                 }
                 CUDA_OK(cudaGetLastError());
                 dim3 gv((p.out_w + 127) / 128, std::min<uint32_t>(p.out_h, 65535u), (unsigned)cnt);
@@ -1108,18 +1136,21 @@ int check_rows(const ifb200_resample_desc& r, int32_t f, size_t i, const char* w
 // (null: all identity): every plan -- of the oriented geometry, in_w and in_h swapped for 5..8 -- is built before anything is
 // enqueued; then the identity jobs go through enqueue_locked exactly as ifb200_batch_enqueue / _rows send them, and the others
 // through its oriented forms.
+// plan (enqueue_profiled_locked): the jobs' profile plans, null for an identity plan.
 void enqueue_oriented_split(ifb200_batch* b, const ifb200_resample_desc* draws, const int32_t* orientation, const int32_t* src, size_t n,
-                            cudaStream_t st) {
+                            cudaStream_t st, const ifb200_profile_plan* const* plan = nullptr) {
     std::vector<ifb200_resample_desc> plain, turned;
     std::vector<int32_t> flags, plain_src, turned_src;
+    std::vector<const ifb200_profile_plan*> plain_plan, turned_plan;
     for (size_t i = 0; i < n; ++i) {
         const int32_t o = orientation ? orientation[i] : 1;
         const int32_t s = src ? src[i] : HV_SRC_BGRA;
-        if (ori_class(o) == HV_ORI_NONE) { plain.push_back(draws[i]); plain_src.push_back(s); continue; }
+        if (ori_class(o) == HV_ORI_NONE) { plain.push_back(draws[i]); plain_src.push_back(s); plain_plan.push_back(plan ? plan[i] : nullptr); continue; }
         ifb200_resample_desc od = draws[i];
         if (ori_class(o) == HV_ORI_TRANSPOSE) std::swap(od.in_w, od.in_h);
         turned.push_back(od);
         turned_src.push_back(s);
+        turned_plan.push_back(plan ? plan[i] : nullptr);
         flags.push_back(o);
     }
     {
@@ -1129,8 +1160,8 @@ void enqueue_oriented_split(ifb200_batch* b, const ifb200_resample_desc* draws, 
         b->prebuild_plans(turned.data(), turned.size());
         for (const auto& od : turned) b->plan_for(od);
     }
-    enqueue_locked(b, plain.data(), plain.size(), st, nullptr, src ? plain_src.data() : nullptr);
-    enqueue_locked(b, turned.data(), turned.size(), st, flags.data(), src ? turned_src.data() : nullptr);
+    enqueue_locked(b, plain.data(), plain.size(), st, nullptr, src ? plain_src.data() : nullptr, plan ? plain_plan.data() : nullptr);
+    enqueue_locked(b, turned.data(), turned.size(), st, flags.data(), src ? turned_src.data() : nullptr, plan ? turned_plan.data() : nullptr);
 }
 
 // ifb200_batch_enqueue_oriented: every descriptor is checked as stored, then enqueue_oriented_split.
@@ -1172,6 +1203,36 @@ void enqueue_rows_oriented_locked(ifb200_batch* b, const ifb200_rows_oriented_re
         draws[i] = d[i].draw; flags[i] = d[i].orientation;
     }
     enqueue_oriented_split(b, draws.data(), flags.data(), src.data(), n, st);
+}
+
+// ifb200_batch_enqueue_profiled: every descriptor is checked on the source as stored (a BGRA window as ifb200_batch_enqueue_oriented
+// checks it, rows with check_rows) and every distinct profile planned once (ifb::ProfilePlans), then enqueue_oriented_split with the
+// plans; identity plans run as the matching entry runs them.
+void enqueue_profiled_locked(ifb200_batch* b, const ifb200_profiled_resample_desc* d, size_t n, cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    if (n == 0) return;
+    std::vector<ifb200_resample_desc> draws(n);
+    std::vector<int32_t> src(n), flags(n);
+    std::vector<uint32_t> plan_of(n);
+    ifb::ProfilePlans pp;
+    for (size_t i = 0; i < n; ++i) {
+        if (d[i].format == IFB200_PROFILE_SRC_BGRA) {
+            int code = 0;
+            const std::string why = ifb::resample_check(d[i].draw, &code);
+            if (!why.empty()) IFB_THROW(code, "profiled resample job %zu: %s", i, why.c_str());
+            src[i] = HV_SRC_BGRA;
+        } else {
+            src[i] = check_rows(d[i].draw, d[i].format, i, "profiled resample", "ifb200_batch_enqueue_profiled (IFB200_PROFILE_SRC_BGRA)");
+        }
+        if (!d[i].profile) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "profiled resample job %zu: null profile pointer", i);
+        std::string why;
+        const int code = pp.add(*d[i].profile, &plan_of[i], &why);
+        if (code != IFB200_OK) IFB_THROW(code, "profiled resample job %zu: %s", i, why.c_str());
+        draws[i] = d[i].draw; flags[i] = d[i].orientation;
+    }
+    std::vector<const ifb200_profile_plan*> plan(n);
+    for (size_t i = 0; i < n; ++i) plan[i] = pp.plans[plan_of[i]].kind == IFB200_PLAN_IDENTITY ? nullptr : &pp.plans[plan_of[i]];
+    enqueue_oriented_split(b, draws.data(), flags.data(), src.data(), n, st, plan.data());
 }
 
 // The argument checks of a BGRA window, shared by the device and the host-buffer form of each operation: a null pointer, or a stride
@@ -2004,6 +2065,9 @@ int ifb200_batch_enqueue_rows_oriented(ifb200_batch* b, const ifb200_rows_orient
     return with_batch(b, stream, err, cap, [&](cudaStream_t st) { enqueue_rows_oriented_locked(b, d, n, st); });
 }
 
+int ifb200_batch_enqueue_profiled(ifb200_batch* b, const ifb200_profiled_resample_desc* d, size_t n, void* stream, char* err, size_t cap) {
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { enqueue_profiled_locked(b, d, n, st); });
+}
 int ifb200_batch_color_matrix(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride, const float m[25],
                               void* stream, char* err, size_t cap) {
     return with_batch(b, stream, err, cap, [&](cudaStream_t st) { color_matrix_locked(b, dev_px, w, h, stride, m, st); });

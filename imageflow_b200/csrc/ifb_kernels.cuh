@@ -35,6 +35,7 @@ namespace ifbk {
 // ---------------------------------------------------------------- scalar helpers
 #include "ifb_lut.cuh"
 #include "ifb_finish.cuh"
+#include "ifb_profile_step.cuh"
 
 // ---------------------------------------------------------------- generic two-kernel path
 // Any geometry / filter.  H pass writes a float4 intermediate [in_h][out_w]; V pass + store epilogue read it.
@@ -76,9 +77,12 @@ __device__ __forceinline__ uint32_t rows_tap_bgra(const uint8_t* p) {
     if constexpr (BPP == 3) return (uint32_t)__ldg(p + 2) | ((uint32_t)__ldg(p + 1) << 8) | ((uint32_t)__ldg(p) << 16) | 0xff000000u;
     else return __byte_perm(__ldg(reinterpret_cast<const uint32_t*>(p)), 0u, 0x3012);
 }
-template <bool TR, int BPP = 0>
+// PROF != PF_IDENTITY (ifb200_batch_enqueue_profiled): every tap through pf_step under the plan `prof` first, its tables read
+// through __ldg (flag 1 is the form without flips).
+template <bool TR, int BPP = 0, int PROF = PF_IDENTITY>
 __global__ void __launch_bounds__(128) hpass_oriented_kernel(const JobDev* __restrict__ jobs, Tables tb, AxisDev ah, uint32_t in_w,
-                                                             uint32_t in_h, uint32_t out_w, float4* __restrict__ inter) {
+                                                             uint32_t in_h, uint32_t out_w, float4* __restrict__ inter,
+                                                             const ProfDev* __restrict__ prof) {
     constexpr size_t kPx = BPP == 0 ? 4 : BPP;                   // bytes per stored pixel
     const JobDev& job = jobs[blockIdx.z];
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -103,6 +107,13 @@ __global__ void __launch_bounds__(128) hpass_oriented_kernel(const JobDev* __res
             uint32_t px;                                               // the tap as a BGRA word
             if constexpr (BPP == 0) px = __ldg(reinterpret_cast<const uint32_t*>(line + (size_t)ks * step));
             else px = rows_tap_bgra<BPP>(line + (size_t)ks * step);
+            if constexpr (PROF != PF_IDENTITY) {
+                float m[9];
+#pragma unroll
+                for (int q = 0; q < 9; ++q) m[q] = PROF == PF_MATRIX ? __ldg(prof->m + q) : 0.0f;
+                px = pf_step<0u>(px, (uint32_t)PROF, m, [&](int c, uint32_t v) { return __ldg(&prof->trc[c][v]); },
+                                 [&](uint32_t v) { return (uint32_t)__ldg(prof->gray + v); }, [&](float x) { return lut_encode(tb.lut16k, x); });
+            }
             const float wt = __ldg(w + (k - l));
             float pb = __ldg(T + (px & 0xffu)), pg = __ldg(T + ((px >> 8) & 0xffu)), pr = __ldg(T + ((px >> 16) & 0xffu)), pa = 0.0f;
             if (am) {

@@ -395,34 +395,34 @@ int profile_plan(const ifb200_source_profile& p, ifb200_profile_plan* plan, std:
     return st.code;
 }
 
+int ProfilePlans::add(const ifb200_source_profile& p, uint32_t* index, std::string* why) {
+    size_t k = 0;
+    while (k < planned.size() && !same_profile(*planned[k], p)) ++k;
+    *index = (uint32_t)k;
+    if (k < planned.size()) return IFB200_OK;
+    plans.emplace_back();
+    planned.push_back(&p);
+    return profile_plan(p, &plans.back(), why);
+}
+
 std::string transform_to_srgb_prepare(const ifb200_to_srgb_desc* d, size_t n, PfWork& wk, int* code) {
-    std::vector<ifb200_profile_plan> plans;
-    std::vector<const ifb200_source_profile*> planned;      // the profile each plan was made from
+    ProfilePlans pp;
     std::vector<uint32_t> plan_of(n, 0);
     for (size_t i = 0; i < n; ++i) {
         if (d[i].w == 0 || d[i].h == 0) continue;
         std::string why = check_desc(d[i], code);
-        if (why.empty()) {
-            size_t k = 0;
-            while (k < planned.size() && !same_profile(*planned[k], *d[i].profile)) ++k;
-            if (k == planned.size()) {
-                plans.emplace_back();
-                *code = profile_plan(*d[i].profile, &plans.back(), &why);
-                planned.push_back(d[i].profile);
-            }
-            plan_of[i] = (uint32_t)k;
-        }
+        if (why.empty()) *code = pp.add(*d[i].profile, &plan_of[i], &why);
         if (!why.empty()) return "transform to srgb job " + std::to_string(i) + ": " + why;
     }
     *code = IFB200_OK;
     for (size_t i = 0; i < n; ++i) {
         if (d[i].w == 0 || d[i].h == 0) continue;
         const bool bgra = d[i].format == IFB200_PROFILE_SRC_BGRA;
-        if (bgra && d[i].src == d[i].dst && plans[plan_of[i]].kind == IFB200_PLAN_IDENTITY) continue;   // nothing to write
+        if (bgra && d[i].src == d[i].dst && pp.plans[plan_of[i]].kind == IFB200_PLAN_IDENTITY) continue;   // nothing to write
         pixel_convert_plan(as_pixel_convert(d[i]), wk.pc);
         wk.plan_of.push_back(plan_of[i] | (bgra ? kPfBgra : 0u));
     }
-    wk.plans = std::move(plans);
+    wk.plans = std::move(pp.plans);
     return "";
 }
 

@@ -25,6 +25,15 @@ struct PfWork {
 // IFB200_OK and *plan filled, or IFB200_ERR_NOT_IMPLEMENTED / IFB200_ERR_INVALID_ARGUMENT with *why.
 int profile_plan(const ifb200_source_profile& p, ifb200_profile_plan* plan, std::string* why);
 
+// The plans of one call's profiles: identical profiles (compared byte for byte) share one plan, planned once.  Used by
+// ifb200_batch_transform_to_srgb and ifb200_batch_enqueue_profiled.
+struct ProfilePlans {
+    std::vector<ifb200_profile_plan> plans;
+    std::vector<const ifb200_source_profile*> planned;   // the profile each plan was made from
+    // *index = the plan of p, planned now if no identical profile has been.  IFB200_OK, or the planner's status with *why.
+    int add(const ifb200_source_profile& p, uint32_t* index, std::string* why);
+};
+
 // Checks every descriptor of one call and plans every distinct profile, then plans the items into wk.  Empty on success; else
 // "transform to srgb job i: <why>" for the first rejected job, with *code = its status, and nothing planned.
 std::string transform_to_srgb_prepare(const ifb200_to_srgb_desc* d, size_t n, PfWork& wk, int* code);

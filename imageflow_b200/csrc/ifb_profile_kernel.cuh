@@ -14,22 +14,19 @@
 //   gray    B, G, R = map[B]
 // Alpha passes unchanged (255 from RGB24 and Gray8 rows, as to_bgra gives).
 
+#include "ifb_profile_step.cuh"
+static_assert(PF_IDENTITY == (uint32_t)IFB200_PLAN_IDENTITY && PF_MATRIX == (uint32_t)IFB200_PLAN_MATRIX && PF_GRAY == (uint32_t)IFB200_PLAN_GRAY, "plan kinds");
+
 struct PfShared {
     float trc[3][256];
     uint8_t gray[256];
 };
 
-// one BGRA pixel through the plan
+// one BGRA pixel through the plan (pf_step)
 __device__ __forceinline__ uint32_t pf_pixel(uint32_t p, const PfShared& s, uint32_t kind, const float (&m)[9],
                                              const uint8_t* __restrict__ lut16k) {
-    if (kind == IFB200_PLAN_GRAY) return (uint32_t)s.gray[p & 0xffu] * 0x010101u | (p & 0xff000000u);
-    if (kind != IFB200_PLAN_MATRIX) return p;
-    const float r = s.trc[0][(p >> 16) & 0xffu], g = s.trc[1][(p >> 8) & 0xffu], b = s.trc[2][p & 0xffu];
-    uint32_t o[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c)
-        o[c] = lut_encode(lut16k, __fadd_rn(__fadd_rn(__fmul_rn(m[3 * c], r), __fmul_rn(m[3 * c + 1], g)), __fmul_rn(m[3 * c + 2], b)));
-    return o[2] | o[1] << 8 | o[0] << 16 | (p & 0xff000000u);
+    return pf_step<0u>(p, kind, m, [&](int c, uint32_t v) { return s.trc[c][v]; }, [&](uint32_t v) { return (uint32_t)s.gray[v]; },
+                       [&](float x) { return lut_encode(lut16k, x); });
 }
 
 // group g of destination row y: to_bgra of the source as pixel_convert_kernel computes it (opaque = 0; a BGRA source as it is), then

@@ -9,7 +9,8 @@ from typing import Optional, Sequence
 
 import numpy as np
 
-from ._lib import (CanvasDesc, ColorDesc, ColorStep, DetectContentDesc, OrientDesc, OrientedResampleDesc, PixelConvertDesc, ProfilePlan, ResampleDesc,
+from ._lib import (CanvasDesc, ColorDesc, ColorStep, DetectContentDesc, OrientDesc, OrientedResampleDesc, PixelConvertDesc, ProfilePlan,
+                   ProfiledResampleDesc, ResampleDesc,
                    RoundCornersDesc, RowsOrientedResampleDesc, RowsResampleDesc, SourceProfileDesc, ToSrgbDesc, WatermarkDesc, lib)
 
 
@@ -1379,6 +1380,52 @@ class Batch:
         an argument is rejected."""
         descs, keep = self.make_rows_oriented_descs(jobs)
         self.enqueue_rows_oriented(descs, stream, keep)
+
+    def make_profiled_descs(self, jobs):
+        """jobs: iterable of (source, canvas BitmapWindow, ScaleAndRenderParams, profile[, orientation[, color_matrix[,
+        alpha_meaningful]]]); `source` a BGRA BitmapWindow or decoder rows as make_rows_descs takes them (3 or 4 channels), as stored;
+        `profile` its SourceProfile; `orientation` the EXIF flag (default 1).  alpha_meaningful defaults as in make_rows_oriented_descs
+        (rows); a BitmapWindow carries its own."""
+        jobs = list(jobs)
+        arr = (ProfiledResampleDesc * len(jobs))()
+        keep = []
+        for i, j in enumerate(jobs):
+            profile = j[3]
+            if not isinstance(profile, SourceProfile):
+                raise FlowError(ErrorKind.InvalidArgument, f"profiled resample job {i}: not a SourceProfile: {profile!r}")
+            cm = j[5] if len(j) > 5 else None
+            if isinstance(j[0], BitmapWindow):
+                src, fmt = j[0], PROFILE_SRC_BGRA
+                if len(j) > 6 and j[6] is not None:
+                    src = BitmapWindow(src.ptr, src.w, src.h, src.stride, alpha_meaningful=bool(j[6]), _keep=src._keep)
+            else:
+                rows = PixelRows.of(j[0])
+                am = (rows.channels == 4) if len(j) < 7 or j[6] is None else bool(j[6])
+                src = BitmapWindow(rows.ptr, rows.w, rows.h, rows.stride, alpha_meaningful=am, _keep=rows._keep)
+                fmt = self._ROWS_FORMAT.get(rows.channels, -1)
+            _fill_desc(arr[i].draw, src, j[1], j[2], cm, keep)
+            arr[i].format = fmt
+            arr[i].orientation = int(j[4]) if len(j) > 4 and j[4] is not None else 1
+            pd = profile._desc()
+            arr[i].profile = C.cast(C.byref(pd), C.c_void_p)
+            keep.append((pd, profile, src._keep))
+        keep.append([j[1]._keep for j in jobs])                         # the bitmaps stay alive until sync() / close()
+        return arr, keep
+
+    def enqueue_profiled(self, descs, stream=None, keep=None) -> None:
+        if keep:
+            self._keep.append(keep)
+        buf = C.create_string_buffer(512)
+        _check(lib().ifb200_batch_enqueue_profiled(self._h, descs, len(descs), self._stream(stream), buf, 512), buf)
+
+    def scale_and_render_profiled(self, jobs, stream=None) -> None:
+        """scale_and_render(orient(transform_to_srgb(to_bgra(source), profile), orientation), canvas, params) on DEVICE frames without
+        the sRGB, BGRA or oriented frame being written: jobs as make_profiled_descs takes them -- e.g. nvJPEG's (H, W, 3) RGB tensor, the
+        photo's Display P3 ICC profile and its EXIF flag.  Byte for byte what transform_to_srgb followed by scale_and_render_oriented /
+        _rows_oriented gives.  Every profile is planned before anything is enqueued: an unsupported one raises MethodNotImplemented
+        (route it with source_profile_plan first), and nothing is written when an argument is rejected.  Asynchronous on `stream`."""
+        descs, keep = self.make_profiled_descs(jobs)
+        self.enqueue_profiled(descs, stream, keep)
 
     def color_matrix(self, dev_ptr: int, w: int, h: int, stride: int, m, stream=None) -> None:
         mm = np.ascontiguousarray(m, np.float32).reshape(25)

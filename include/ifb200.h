@@ -372,6 +372,22 @@ typedef struct ifb200_rows_oriented_resample_desc {
     int32_t orientation;
 } ifb200_rows_oriented_resample_desc;
 
+/* One resample of a frame with a colour profile: scale_and_render(orient(transform_to_srgb(to_bgra(draw.in, format), profile),
+ * orientation), canvas, params), byte for byte as ifb200_batch_transform_to_srgb followed by the matching resample entry, without the
+ * sRGB frame, the BGRA frame or the oriented frame ever being written -- a Display P3 phone photo straight into a thumbnail.
+ *   draw         the source as stored; every other field as in ifb200_batch_enqueue.
+ *   format       IFB200_PROFILE_SRC_BGRA (a BGRA window: the rules of ifb200_batch_enqueue_oriented), or IFB200_PIXEL_RGB24_TO_BGRA /
+ *                IFB200_PIXEL_RGBA_TO_BGRA (decoder rows: the rules of ifb200_batch_enqueue_rows_oriented).  Gray8 and GrayAlpha8
+ *                rows are refused.
+ *   orientation  EXIF flag as in ifb200_oriented_resample_desc; values other than 2..8 are the identity.
+ *   profile      HOST pointer, read before the call returns; the semantics of ifb200_batch_transform_to_srgb. */
+typedef struct ifb200_profiled_resample_desc {
+    ifb200_resample_desc draw;
+    int32_t format;
+    int32_t orientation;
+    const ifb200_source_profile* profile;
+} ifb200_profiled_resample_desc;
+
 /* One frame of ifb200_batch_detect_content_many: detect_content (graphics/whitespace.rs:284-331) of the DEVICE BGRA window px
  * (w x h, row pitch `stride` bytes), grayscale Bgra32 when alpha_meaningful != 0 else Bgr32, edges where the Scharr value exceeds
  * `threshold`.  The limits are those of ifb200_batch_detect_content: a non-empty window, w and h below 2^31, threshold below 2^31. */
@@ -420,6 +436,17 @@ int  ifb200_batch_enqueue_rows(ifb200_batch* b, const ifb200_rows_resample_desc*
  * these jobs too. */
 int  ifb200_batch_enqueue_rows_oriented(ifb200_batch* b, const ifb200_rows_oriented_resample_desc* d, size_t n, void* cuda_stream,
                                         char* err, size_t err_cap);
+/* n resamples of DEVICE frames with colour profiles (ifb200_profiled_resample_desc), asynchronous on `cuda_stream`, as
+ * ifb200_batch_enqueue.  The transform to sRGB happens in the resample's source reads, per source pixel in the ring kernel and per tap
+ * in the generic pair's H pass.  Down-scales run the streaming ring kernel under the rules of the matching entry; up-scales, 1:1,
+ * other windows, forms that are not compiled (the general store epilogue: a compositing mode other than ReplaceSelf or a colour
+ * matrix) and IFB200_OPT_FORCE_GENERIC run the generic pair.  Jobs whose profile plans to IFB200_PLAN_IDENTITY run exactly as
+ * the matching entry runs them.  Every descriptor is checked and every distinct profile planned once before anything is enqueued,
+ * so an error ("profiled resample job i: ...", with the planner's status: IFB200_ERR_NOT_IMPLEMENTED for a profile the GPU does not
+ * transform -- route such frames with ifb200_source_profile_plan first) means nothing is written.  One ring launch per geometry,
+ * kernel form and profile.  ifb200_batch_fused_jobs / ifb200_batch_generic_jobs count these jobs too. */
+int  ifb200_batch_enqueue_profiled(ifb200_batch* b, const ifb200_profiled_resample_desc* d, size_t n, void* cuda_stream,
+                                   char* err, size_t err_cap);
 int  ifb200_batch_color_matrix(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride,
                                const float m[25], void* cuda_stream, char* err, size_t err_cap);
 int  ifb200_batch_apply_matte(ifb200_batch* b, uint8_t* dev_px, uint32_t w, uint32_t h, uint32_t stride,
