@@ -24,6 +24,7 @@
 #include "ifb_color.h"             // ClJob / ClSeg: planned on the host, read by the colour-chain kernels
 #include "ifb_watermark.h"         // WmJob / WmGroup: planned on the host, read by watermark_composite_kernel
 #include "ifb_pixel_convert.h"     // PcItem: planned on the host, read by pixel_convert_kernel
+#include "ifb_ycbcr.h"             // YcItem: planned on the host, read by ycbcr_to_bgra_kernel
 #include "ifb_profile.h"           // PfWork: planned on the host, read by transform_to_srgb_kernel
 #include "ifb_whitespace.h"        // WsSeg / WsJob / WsColumn: planned on the host, read by the detect_content_many kernels
 
@@ -404,6 +405,7 @@ __global__ void __launch_bounds__(256) apply_byte_maps_bgra8_kernel(uint8_t* __r
 
 // ---------------------------------------------------------------- pixel formats at the graph's edges (RGB24, RGBA, Gray, GrayAlpha <-> BGRA); own file for tests/cpu_emu
 #include "ifb_pixel_convert_kernel.cuh"
+#include "ifb_ycbcr_kernel.cuh"
 
 // ---------------------------------------------------------------- colour profiles to sRGB (matrix-shaper ICC, gray ICC, gAMA+cHRM, CICP); own file for tests/cpu_emu
 #include "ifb_profile_kernel.cuh"

@@ -13,8 +13,10 @@ const char* op_name(int32_t op) {
     return names[op];
 }
 
-// 16-byte groups per destination row of `bytes` bytes starting at `row0`, for rows `stride` bytes apart: the rows' phases modulo 16
-// are row0's plus multiples of gcd(stride, 16), so the latest any row starts in its first group is (row0 mod g) + 16 - g.
+}  // namespace
+
+// The rows' phases modulo 16 are row0's plus multiples of gcd(stride, 16), so the latest any row starts in its first group is
+// (row0 mod g) + 16 - g.
 uint32_t dst_groups_per_row(const uint8_t* row0, uint32_t stride, uint64_t bytes) {
     uint32_t g = 16;
     while (stride % g) g >>= 1;
@@ -22,7 +24,10 @@ uint32_t dst_groups_per_row(const uint8_t* row0, uint32_t stride, uint64_t bytes
     return (uint32_t)std::min<uint64_t>((late + bytes + 15) / 16, 0xffffffffull);
 }
 
-}  // namespace
+void push_first_cta(std::vector<uint32_t>& first, uint64_t ctas) {
+    if (first.empty()) first.push_back(0);
+    first.push_back((uint32_t)std::min<uint64_t>(first.back() + ctas, 0xffffffffull));
+}
 
 uint32_t pixel_src_bytes(int32_t op) {
     switch (op) {
@@ -68,10 +73,8 @@ void pixel_convert_plan(const ifb200_pixel_convert_desc& d, PcWork& wk) {
     it.src = d.src; it.dst = d.dst; it.src_stride = d.src_stride; it.dst_stride = d.dst_stride; it.w = d.w; it.h = d.h;
     it.op = (uint32_t)d.op; it.opaque = d.opaque ? 1u : 0u;
     it.groups = dst_groups_per_row(d.dst, d.dst_stride, (uint64_t)d.w * pixel_dst_bytes(d.op));
-    if (wk.first.empty()) wk.first.push_back(0);
     wk.items.push_back(it);
-    const uint64_t ctas = ((uint64_t)it.groups * it.h + kPcCtaGroups - 1) / kPcCtaGroups;
-    wk.first.push_back((uint32_t)std::min<uint64_t>(wk.first.back() + ctas, 0xffffffffull));
+    push_first_cta(wk.first, ((uint64_t)it.groups * it.h + kPcCtaGroups - 1) / kPcCtaGroups);
 }
 
 std::string pixel_convert_prepare(const ifb200_pixel_convert_desc* d, size_t n, PcWork& wk, int* code) {

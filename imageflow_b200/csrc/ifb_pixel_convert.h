@@ -29,6 +29,13 @@ struct PcWork {
     uint64_t ctas() const { return first.empty() ? 0 : first.back(); }
 };
 
+// The plan shape every flat launch over whole-window items shares (pixel_convert, ycbcr_to_bgra): 16-byte groups per destination row
+// of `bytes` bytes starting at `row0`, rows `stride` bytes apart, so that a row at any phase its stride allows is covered; and the
+// first-CTA prefix, extended by an item of `ctas` CTAs (a leading 0 and a trailing total, saturating at 2^32 - 1).  The kernels find
+// their item with pc_item_of (ifb_pixel_convert_kernel.cuh).
+uint32_t dst_groups_per_row(const uint8_t* row0, uint32_t stride, uint64_t bytes);
+void push_first_cta(std::vector<uint32_t>& first, uint64_t ctas);
+
 // Bytes per pixel of op's source and destination (0 for an unknown op).
 uint32_t pixel_src_bytes(int32_t op);
 uint32_t pixel_dst_bytes(int32_t op);

@@ -137,14 +137,20 @@ __device__ __forceinline__ void pc_group(const ifb::PcItem& it, uint32_t y, uint
     pc_store(drow + q0, out, (uint32_t)(lo - q0), (uint32_t)(hi - q0));
 }
 
-__global__ void __launch_bounds__(256) pixel_convert_kernel(const ifb::PcItem* __restrict__ items, const uint32_t* __restrict__ first,
-                                                            uint32_t n) {
-    uint32_t lo = 0, hi = n;                                     // the item i with first[i] <= blockIdx.x < first[i + 1]
+// the item i of n with first[i] <= blockIdx.x < first[i + 1] (ifb::push_first_cta's prefix)
+__device__ __forceinline__ uint32_t pc_item_of(const uint32_t* __restrict__ first, uint32_t n) {
+    uint32_t lo = 0, hi = n;
     while (hi - lo > 1) {
         const uint32_t mid = (lo + hi) / 2;
         if (first[mid] <= blockIdx.x) lo = mid;
         else hi = mid;
     }
+    return lo;
+}
+
+__global__ void __launch_bounds__(256) pixel_convert_kernel(const ifb::PcItem* __restrict__ items, const uint32_t* __restrict__ first,
+                                                            uint32_t n) {
+    const uint32_t lo = pc_item_of(first, n);
     const ifb::PcItem it = items[lo];
     const uint64_t total = (uint64_t)it.groups * it.h, k0 = (uint64_t)(blockIdx.x - first[lo]) * ifb::kPcCtaGroups;
     if (k0 >= total) return;

@@ -11,7 +11,7 @@ import numpy as np
 
 from ._lib import (CanvasDesc, ColorDesc, ColorStep, DetectContentDesc, OrientDesc, OrientedResampleDesc, PixelConvertDesc, ProfilePlan,
                    ProfiledResampleDesc, ResampleDesc,
-                   RoundCornersDesc, RowsOrientedResampleDesc, RowsResampleDesc, SourceProfileDesc, ToSrgbDesc, WatermarkDesc, lib)
+                   RoundCornersDesc, RowsOrientedResampleDesc, RowsResampleDesc, SourceProfileDesc, ToSrgbDesc, WatermarkDesc, YcbcrDesc, lib)
 
 
 class Filter(enum.IntEnum):
@@ -1129,6 +1129,10 @@ class BgraToRgb:
 
 
 _PIXEL_OPS = {c.OP: c for c in (RgbToBgra, RgbaToBgra, GrayToBgra, GrayAlphaToBgra, BgraToRgb)}
+_YCBCR_DESC_DTYPE = np.dtype({"names": [n for n, _ in YcbcrDesc._fields_],
+                              "formats": [np.uint64 if t is C.c_void_p else np.dtype(t) for n, t in YcbcrDesc._fields_],
+                              "offsets": [getattr(YcbcrDesc, n).offset for n, _ in YcbcrDesc._fields_],
+                              "itemsize": C.sizeof(YcbcrDesc)})
 _PIXEL_DESC_DTYPE = np.dtype({"names": [n for n, _ in PixelConvertDesc._fields_],
                               "formats": [np.uint64 if t is C.c_void_p else np.dtype(t) for n, t in PixelConvertDesc._fields_],
                               "offsets": [getattr(PixelConvertDesc, n).offset for n, _ in PixelConvertDesc._fields_],
@@ -1141,6 +1145,37 @@ def pixel_op_for(channels: int, to_bgra: bool = True):
     if channels not in ops:
         raise FlowError(ErrorKind.InvalidArgument, f"no conversion {'from' if to_bgra else 'to'} {channels}-channel rows")
     return ops[channels]
+
+
+# ---------------------------------------------------------------- a JPEG's Y, Cb, Cr planes into BGRA (Batch.ycbcr_to_bgra)
+YCBCR_444, YCBCR_422, YCBCR_420 = 0, 1, 2                          # include/ifb200.h enum ifb200_ycbcr_sampling
+
+
+def ycbcr_chroma_shape(sampling: int, w: int, h: int) -> tuple:
+    """(rows, columns) of the Cb and Cr planes of a w x h frame at `sampling` (YCBCR_444, YCBCR_422 or YCBCR_420)"""
+    if sampling not in (YCBCR_444, YCBCR_422, YCBCR_420):
+        raise FlowError(ErrorKind.InvalidArgument, f"unknown YCbCr sampling {sampling!r}: YCBCR_444 (0), YCBCR_422 (1) or YCBCR_420 (2)")
+    if sampling == YCBCR_444:
+        return h, w
+    return ((h + 1) // 2 if sampling == YCBCR_420 else h), (w + 1) // 2
+
+
+def _plane(x) -> "PixelRows":
+    """PixelRows of one 8-bit plane: PixelRows with one channel, or a uint8 (H, W) or (H, W, 1) tensor or array"""
+    if not isinstance(x, PixelRows) and len(getattr(x, "shape", ())) == 2:
+        if isinstance(x, np.ndarray):
+            ptr, strides, ok = x.ctypes.data, x.strides, x.dtype == np.uint8
+        else:
+            import torch
+            ptr, strides, ok = x.data_ptr(), x.stride(), x.dtype == torch.uint8
+        if not ok or strides[1] != 1 or strides[0] < 0:
+            raise FlowError(ErrorKind.InvalidArgument, f"a YCbCr plane is (H, W) uint8 with unit column stride; got {x.dtype}, strides "
+                                                       f"{tuple(strides)}")
+        return PixelRows(ptr, x.shape[1], x.shape[0], strides[0], 1, x)
+    p = PixelRows.of(x)
+    if p.channels != 1:
+        raise FlowError(ErrorKind.InvalidArgument, f"a YCbCr plane has one channel, not {p.channels}")
+    return p
 
 
 # ---------------------------------------------------------------- colour profiles to sRGB (Batch.transform_to_srgb)
@@ -1592,6 +1627,37 @@ class Batch:
             out.append(dst)
         self._keep.append([(s._keep, d._keep) for s, d in zip(srcs, dsts)])
         return out
+
+    def ycbcr_to_bgra(self, jobs, stream=None) -> list:
+        """A JPEG's colour stage on DEVICE planes -- libjpeg-turbo's fancy upsampling and YCbCr -> RGB, byte for byte as it decodes into
+        JCS_EXT_BGRA -- all jobs in one kernel launch (none when no job has pixels), asynchronous on `stream`.  jobs: iterable of
+        (y, cb, cr, sampling, dst): the planes a GPU decoder hands over (uint8 (H, W) CUDA tensors or one-channel PixelRows, each at
+        any pitch), sampling YCBCR_444, YCBCR_422 or YCBCR_420 -- always given, never inferred: plane shapes cannot tell the samplings
+        apart at widths and heights of 1 and 2 -- and dst a BGRA BitmapWindow (or 4-channel rows) the size of y.  The chroma planes must
+        be ycbcr_chroma_shape(sampling, w, h).  Returns the destinations; a BitmapWindow gets alpha_meaningful = False (alpha is 255).
+        Nothing is changed when an argument is rejected.  Gray JPEGs need no such call: their plane is GrayToBgra's Gray8 rows."""
+        jobs = list(jobs)
+        rows, keep = [], []
+        for y, cb, cr, sampling, dst in jobs:
+            py, pb, pr, t = _plane(y), _plane(cb), _plane(cr), PixelRows.of(dst)
+            ch, cw = ycbcr_chroma_shape(sampling, py.w, py.h)
+            if (pb.h, pb.w) != (ch, cw) or (pr.h, pr.w) != (ch, cw):
+                raise FlowError(ErrorKind.InvalidArgument, f"a {py.w}x{py.h} frame at sampling {sampling} has {cw}x{ch} chroma planes, not "
+                                                           f"{pb.w}x{pb.h} and {pr.w}x{pr.h}")
+            if t.channels != 4 or (t.w, t.h) != (py.w, py.h):
+                raise FlowError(ErrorKind.InvalidArgument, f"ycbcr_to_bgra writes a {py.w}x{py.h} BGRA frame, not {t.w}x{t.h}x{t.channels}")
+            rows.append((sampling, py.ptr, py.stride, pb.ptr, pb.stride, pr.ptr, pr.stride, t.ptr, t.stride, py.w, py.h))
+            keep.append((py._keep, pb._keep, pr._keep, t._keep))
+        a = np.array(rows, _YCBCR_DESC_DTYPE) if rows else np.zeros(0, _YCBCR_DESC_DTYPE)   # one conversion, no per-field ctypes marshalling
+        arr = (YcbcrDesc * len(jobs)).from_buffer(a)
+        buf = C.create_string_buffer(512)
+        _check(lib().ifb200_batch_ycbcr_to_bgra(self._h, arr, len(jobs), self._stream(stream), buf, 512), buf)
+        outs = [j[4] for j in jobs]
+        for o in outs:
+            if isinstance(o, BitmapWindow):
+                o.alpha_meaningful = False
+        self._keep.append(keep)
+        return outs
 
     def transform_to_srgb(self, jobs, stream=None) -> list:
         """transform_to_srgb(to_bgra(src), profile) (codecs/cms.rs:68 under the moxcms backend) on DEVICE frames, all jobs in one kernel

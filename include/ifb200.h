@@ -293,6 +293,32 @@ typedef struct ifb200_pixel_convert_desc {
     int32_t        opaque;                  /* != 0: alpha = 255 in a 4-byte output */
 } ifb200_pixel_convert_desc;
 
+/* One JPEG frame's colour stage: the Y, Cb and Cr planes a GPU JPEG decoder hands over (nvJPEG's NVJPEG_OUTPUT_YUV, at the file's
+ * chroma subsampling) into a BGRA frame, byte for byte as libjpeg-turbo decodes into JCS_EXT_BGRA with its defaults (the reference's
+ * mozjpeg decoder, codecs/mozjpeg_decoder.rs): fancy chroma upsampling, then the fixed-point YCbCr -> RGB tables.  Per pixel, with
+ * y, cb, cr the samples after upsampling:
+ *   R = clamp(y + ((91881 (cr - 128) + 32768) >> 16))                      FIX(1.40200)
+ *   G = clamp(y + ((-22554 (cb - 128) + 32768 - 46802 (cr - 128)) >> 16))  FIX(0.34414), FIX(0.71414)
+ *   B = clamp(y + ((116130 (cb - 128) + 32768) >> 16))                     FIX(1.77200)
+ * with >> arithmetic and clamp to 0..255; alpha is 255.  Upsampling, neighbours clamped to the plane (edge rows and columns repeated):
+ *   444  none: the chroma planes are w x h.
+ *   422  chroma ceil(w/2) x h; output column 2i = (3 c[i] + c[i-1] + 1) >> 2, 2i+1 = (3 c[i] + c[i+1] + 2) >> 2 (h2v1_fancy_upsample).
+ *   420  chroma ceil(w/2) x ceil(h/2); column sums s = 3 c[j] + c[j-1] for output row 2j and 3 c[j] + c[j+1] for row 2j+1, then
+ *        output column 2i = (3 s[i] + s[i-1] + 8) >> 4, 2i+1 = (3 s[i] + s[i+1] + 7) >> 4 (h2v2_fancy_upsample).
+ * A chroma plane one or two columns wide is replicated instead (libjpeg-turbo runs the fancy forms only above two columns).  Planes
+ * may sit at any byte address with any pitch that holds a row; the destination is 4-byte aligned.  A grayscale JPEG needs none of
+ * this: its one plane is Gray8 rows, and IFB200_PIXEL_GRAY_TO_BGRA is libjpeg's gray -> BGRA.  4:4:0, 4:1:1, CMYK / YCCK and
+ * Adobe-transform-0 (RGB-coded) JPEGs are not covered. */
+enum ifb200_ycbcr_sampling { IFB200_YCBCR_444 = 0, IFB200_YCBCR_422 = 1, IFB200_YCBCR_420 = 2 };
+typedef struct ifb200_ycbcr_desc {
+    int32_t        sampling;                /* enum ifb200_ycbcr_sampling */
+    const uint8_t* y;  uint32_t y_stride;   /* w x h luma */
+    const uint8_t* cb; uint32_t cb_stride;  /* chroma planes at the sampling's size; each plane has its own pitch */
+    const uint8_t* cr; uint32_t cr_stride;
+    uint8_t*       dst; uint32_t dst_stride;   /* w x h BGRA: 4-byte aligned pointer and stride */
+    uint32_t       w, h;
+} ifb200_ycbcr_desc;
+
 /* A decoder's colour profile (the reference's SourceProfile, codecs/source_profile.rs:7-41, CMYK excluded) and the transform of a
  * frame to sRGB under it: transform_to_srgb(to_bgra(src, format), profile) as codecs/moxcms_transform.rs runs it with
  * lut_transform_opts() (relative colorimetric), for the profiles whose transform is a matrix-shaper.  Kinds:
@@ -522,6 +548,13 @@ int  ifb200_batch_watermark(ifb200_batch* b, const ifb200_watermark_desc* d, siz
  * enqueued, so an error means nothing is written.  There is no host-buffer variant: on host rows the decoders' own loop is cheaper than
  * the trip over PCIe. */
 int  ifb200_batch_pixel_convert(ifb200_batch* b, const ifb200_pixel_convert_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
+/* JPEG colour stages (ifb200_ycbcr_desc) of n DEVICE frames in ONE kernel launch, none when no job has pixels; each destination byte is
+ * written once and nothing outside the planes and the destination window is read or written.  Asynchronous on `cuda_stream`.  No job
+ * may write what another job of the same call reads or writes (not checked).  Every descriptor is checked before anything is planned or
+ * enqueued ("ycbcr job i: <why>", IFB200_ERR_INVALID_ARGUMENT: a null plane or destination, a stride smaller than its plane's row, an
+ * unknown sampling, a misaligned destination, a destination that overlaps a plane of its job), so an error means nothing is written.
+ * A job of zero area is skipped unchecked.  There is no host-buffer variant. */
+int  ifb200_batch_ycbcr_to_bgra(ifb200_batch* b, const ifb200_ycbcr_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
 /* Colour profiles to sRGB (ifb200_to_srgb_desc, ifb200_source_profile) on n DEVICE windows in ONE kernel launch, none when no job
  * writes a pixel (SRGB jobs in place, zero-area jobs); asynchronous on `cuda_stream`.  Each destination byte is written once and
  * nothing outside the two windows is read.  Every descriptor is checked and every profile planned before anything is enqueued, so an
