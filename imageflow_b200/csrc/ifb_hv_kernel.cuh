@@ -48,7 +48,8 @@ struct HvPlanDev {
     int n_strips, n_bands;
     const HvStripDev* strips;
     const HvBandDev* bands;
-    const float* hw;          // [n_strips][hw_stride][AVP]: weight of the open output column in each ring slot, pixel-stream order
+    const float* hw;          // [n_strips][hw_stride][AVP]: weight of the open output column in each ring slot, pixel-stream order (the
+                              // kernel stages each record in register order: ifb_hv_ring_body.inc, H weights of the strip)
     const uint8_t* hdone;     // [n_strips][hw_stride + 64]: output columns completing after this pixel (bits 0..6), V-pass mark (bit 7)
     const float* vw;          // [in_h][AVP]
     const uint8_t* vdone;     // [in_h + 32]
@@ -85,7 +86,7 @@ enum : int { HV_SRC_BGRA = 0, HV_SRC_RGBA = 1, HV_SRC_RGB24 = 2 };
 //                      then read again and again with no refill and no wait
 //   IFB_HV_PROBE_NOPARK  (with IFB_HV_PROBE_MATH) every chunk with one completion runs as the plain form: the arithmetic side
 //                      without the cost of parking a column (the column is counted and its place in the exchange buffer
-//                      advanced; no slot is picked, its values are never stored or cleared)
+//                      advanced; its values are never stored or cleared and the registers do not rotate)
 #ifndef IFB_HV_PROBE_MEM
 #define IFB_HV_PROBE_MEM 0
 #endif
@@ -262,10 +263,6 @@ __device__ __forceinline__ uint32_t ldg_volatile(const uint32_t* p) { return *re
 __device__ __forceinline__ uint32_t lds_u32(uint32_t a) { uint32_t v; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
 }  // namespace hv
 #define IFB_HV_DYNAMIC_SMEM(name_) extern __shared__ __align__(1024) unsigned char name_[]
-#endif
-
-#ifndef IFB_HV_NOFAST
-#define IFB_HV_NOFAST 0                // 1: only the general form of a chunk (A/B builds)
 #endif
 
 // Where a CTA's dynamic shared memory starts in the shared window (the engine sizes the ring kernel's layout with it).
