@@ -30,6 +30,9 @@ Host-side mirror of the reference seam (paths relative to the imageflow checkout
       folded into the resample's source reads with the orientation (Batch.scale_and_render_profiled)
   codecs/mozjpeg_decoder.rs:316-321  the JPEG decoder's colour stage into JCS_EXT_BGRA (libjpeg-turbo's fancy upsampling and YCbCr ->
       RGB) on the Y, Cb and Cr planes a GPU decoder hands over, 4:4:4, 4:2:2 and 4:2:0, batched (Batch.ycbcr_to_bgra)
+  codecs/mozjpeg.rs:93-157  the JPEG encoder's colour stage from JCS_EXT_BGRA (apply_matte, libjpeg-turbo's RGB -> YCbCr and chroma
+      downsampling) into the Y, Cb and Cr planes a GPU encoder takes, 4:4:4, 4:2:2 and 4:2:0, batched (Batch.bgra_to_ycbcr over
+      BgraToYcbcr records; Batch.to_ycbcr for one tensor)
   c_components/lib/codecs_jpeg_idct_fast.c  flow_scale_spatial[_srgb]_NxN (decode-time JPEG block scalers)
 All arithmetic runs in hand-written sm_90a kernels inside libifb200.so (include/ifb200.h);
 this package only marshals arguments.  Nothing here imports the CPU oracle.
@@ -45,8 +48,9 @@ from .graphics import (Batch, apply_matte, BitmapCompositing, BitmapWindow, Erro
                        WhiteBalanceHistogramAreaThresholdSrgb, riapi_color_steps, Watermark, WatermarkConstraintBox, WatermarkConstraintMode, ConstraintGravity, WatermarkDraw,
                        process_constraint, watermark_layout, riapi_watermark_placement, PixelRows, RgbToBgra, RgbaToBgra, GrayToBgra,
                        GrayAlphaToBgra, BgraToRgb, pixel_op_for, CropWhitespace, riapi_trim_steps, crop_whitespace_bounds, SourceProfile,
-                       ProfilePlanResult, source_profile_plan, YCBCR_444, YCBCR_422, YCBCR_420, ycbcr_chroma_shape)
-from ._lib import LIB_PATH, ProfiledResampleDesc, ResampleDesc, RowsOrientedResampleDesc, RowsResampleDesc, YcbcrDesc, lib
+                       ProfilePlanResult, source_profile_plan, YCBCR_444, YCBCR_422, YCBCR_420, ycbcr_chroma_shape,
+                       BgraToYcbcr)
+from ._lib import LIB_PATH, BgraToYcbcrDesc, ProfiledResampleDesc, ResampleDesc, RowsOrientedResampleDesc, RowsResampleDesc, YcbcrDesc, lib
 
 __all__ = [
     "Batch", "apply_matte", "BitmapCompositing", "BitmapWindow", "ErrorKind", "Filter", "FlowError", "ScaleAndRenderParams",
@@ -62,4 +66,5 @@ __all__ = [
     "GrayAlphaToBgra", "BgraToRgb", "pixel_op_for", "CropWhitespace", "riapi_trim_steps", "crop_whitespace_bounds", "SourceProfile",
     "ProfilePlanResult", "source_profile_plan", "LIB_PATH", "ProfiledResampleDesc", "ResampleDesc", "RowsOrientedResampleDesc",
     "RowsResampleDesc", "lib", "YCBCR_444", "YCBCR_422", "YCBCR_420", "ycbcr_chroma_shape", "YcbcrDesc",
+    "BgraToYcbcr", "BgraToYcbcrDesc",
 ]

@@ -24,7 +24,7 @@ SYMBOLS = [
     "ifb200_batch_canvas", "ifb200_batch_orient", "ifb200_batch_color_chain", "ifb200_batch_watermark",
     "ifb200_batch_pixel_convert", "ifb200_batch_enqueue_oriented", "ifb200_batch_enqueue_rows", "ifb200_batch_detect_content_many",
     "ifb200_batch_enqueue_rows_oriented", "ifb200_batch_transform_to_srgb", "ifb200_source_profile_plan",
-    "ifb200_batch_enqueue_profiled", "ifb200_batch_ycbcr_to_bgra",
+    "ifb200_batch_enqueue_profiled", "ifb200_batch_ycbcr_to_bgra", "ifb200_batch_bgra_to_ycbcr",
 ]
 
 
@@ -113,6 +113,15 @@ class YcbcrDesc(C.Structure):
     _fields_ = [
         ("sampling", C.c_int32), ("y", C.c_void_p), ("y_stride", C.c_uint32), ("cb", C.c_void_p), ("cb_stride", C.c_uint32),
         ("cr", C.c_void_p), ("cr_stride", C.c_uint32), ("dst", C.c_void_p), ("dst_stride", C.c_uint32), ("w", C.c_uint32), ("h", C.c_uint32),
+    ]
+
+
+class BgraToYcbcrDesc(C.Structure):
+    """struct ifb200_bgra_to_ycbcr_desc"""
+    _fields_ = [
+        ("sampling", C.c_int32), ("src", C.c_void_p), ("src_stride", C.c_uint32), ("y", C.c_void_p), ("y_stride", C.c_uint32),
+        ("cb", C.c_void_p), ("cb_stride", C.c_uint32), ("cr", C.c_void_p), ("cr_stride", C.c_uint32), ("w", C.c_uint32), ("h", C.c_uint32),
+        ("alpha_meaningful", C.c_int32), ("matte_bgra", C.c_uint8 * 4),
     ]
 
 
@@ -251,6 +260,8 @@ def lib() -> C.CDLL:
     L.ifb200_batch_pixel_convert.restype = C.c_int
     L.ifb200_batch_ycbcr_to_bgra.argtypes = [C.c_void_p, C.POINTER(YcbcrDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_ycbcr_to_bgra.restype = C.c_int
+    L.ifb200_batch_bgra_to_ycbcr.argtypes = [C.c_void_p, C.POINTER(BgraToYcbcrDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
+    L.ifb200_batch_bgra_to_ycbcr.restype = C.c_int
     L.ifb200_batch_transform_to_srgb.argtypes = [C.c_void_p, C.POINTER(ToSrgbDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]
     L.ifb200_batch_transform_to_srgb.restype = C.c_int
     L.ifb200_batch_enqueue_profiled.argtypes = [C.c_void_p, C.POINTER(ProfiledResampleDesc), C.c_size_t, C.c_void_p, C.c_char_p, C.c_size_t]

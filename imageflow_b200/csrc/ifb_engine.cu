@@ -1557,6 +1557,25 @@ void ycbcr_locked(ifb200_batch* b, const ifb200_ycbcr_desc* d, size_t n, cudaStr
     b->launches++;
 }
 
+// The JPEG encoder colour stages of ifb200_batch_bgra_to_ycbcr (ifb_ycbcr_enc.h): every descriptor is checked before anything is
+// planned or enqueued, then all jobs run in ONE launch (none when no job has pixels).  The upload is the items and their first CTAs,
+// O(jobs).
+void bgra_to_ycbcr_locked(ifb200_batch* b, const ifb200_bgra_to_ycbcr_desc* d, size_t n, cudaStream_t st) {
+    if (!d && n) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "null descriptor array");
+    ifb::YeWork wk;
+    int code = 0;
+    const std::string why = ifb::bgra_to_ycbcr_prepare(d, n, wk, &code);
+    if (!why.empty()) IFB_THROW(code, "%s", why.c_str());
+    if (wk.items.empty()) return;
+    if (wk.ctas() > 0x7fffffffu) IFB_THROW(IFB200_ERR_INVALID_ARGUMENT, "too many pixels in one call");
+    DeviceScope dev_scope_(b->device);
+    WorkUpload up(b, st, {part(wk.items), part(wk.first)});
+    bgra_to_ycbcr_kernel<<<(unsigned)wk.ctas(), ifb::kYeThreads, 0, st>>>(up.at<const ifb::YeItem>(0), up.at<const uint32_t>(1),
+                                                                          (uint32_t)wk.items.size(), b->tables);
+    CUDA_OK(cudaGetLastError());
+    b->launches++;
+}
+
 // The profile transforms of ifb200_batch_transform_to_srgb (ifb_profile.h): every descriptor is checked and every distinct profile
 // planned before anything is enqueued, then all jobs run in ONE launch (none when no job writes a pixel).  The upload is the items,
 // their first CTAs and plan indices, and the distinct plans: O(jobs + profiles).
@@ -2137,6 +2156,10 @@ int ifb200_batch_pixel_convert(ifb200_batch* b, const ifb200_pixel_convert_desc*
 
 int ifb200_batch_ycbcr_to_bgra(ifb200_batch* b, const ifb200_ycbcr_desc* d, size_t n, void* stream, char* err, size_t cap) {
     return with_batch(b, stream, err, cap, [&](cudaStream_t st) { ycbcr_locked(b, d, n, st); });
+}
+
+int ifb200_batch_bgra_to_ycbcr(ifb200_batch* b, const ifb200_bgra_to_ycbcr_desc* d, size_t n, void* stream, char* err, size_t cap) {
+    return with_batch(b, stream, err, cap, [&](cudaStream_t st) { bgra_to_ycbcr_locked(b, d, n, st); });
 }
 
 int ifb200_batch_transform_to_srgb(ifb200_batch* b, const ifb200_to_srgb_desc* d, size_t n, void* stream, char* err, size_t cap) {

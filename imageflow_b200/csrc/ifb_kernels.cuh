@@ -25,6 +25,7 @@
 #include "ifb_watermark.h"         // WmJob / WmGroup: planned on the host, read by watermark_composite_kernel
 #include "ifb_pixel_convert.h"     // PcItem: planned on the host, read by pixel_convert_kernel
 #include "ifb_ycbcr.h"             // YcItem: planned on the host, read by ycbcr_to_bgra_kernel
+#include "ifb_ycbcr_enc.h"         // YeItem: planned on the host, read by bgra_to_ycbcr_kernel
 #include "ifb_profile.h"           // PfWork: planned on the host, read by transform_to_srgb_kernel
 #include "ifb_whitespace.h"        // WsSeg / WsJob / WsColumn: planned on the host, read by the detect_content_many kernels
 
@@ -37,6 +38,7 @@ namespace ifbk {
 #include "ifb_lut.cuh"
 #include "ifb_finish.cuh"
 #include "ifb_profile_step.cuh"
+#include "ifb_matte.cuh"
 
 // ---------------------------------------------------------------- generic two-kernel path
 // Any geometry / filter.  H pass writes a float4 intermediate [in_h][out_w]; V pass + store epilogue read it.
@@ -223,9 +225,7 @@ __global__ void __launch_bounds__(256) color_matrix_kernel(uint8_t* __restrict__
 // Encoder-side flatten over a solid colour, in place, linear light (SURVEY.md section 8(f), item 2).
 __global__ void __launch_bounds__(256) apply_matte_kernel(uint8_t* __restrict__ px, uint32_t w, uint32_t h, uint32_t stride,
                                                           uint32_t matte_bgra, Tables tb) {
-    const float a2f = 1.0f / 255.0f;
-    const float ma = __fmul_rn((float)(matte_bgra >> 24), a2f);
-    const float mb = __ldg(tb.t_lin + (matte_bgra & 0xffu)), mg = __ldg(tb.t_lin + ((matte_bgra >> 8) & 0xffu)), mr = __ldg(tb.t_lin + ((matte_bgra >> 16) & 0xffu));
+    const MatteLin ml = matte_lin(matte_bgra, tb);
     const uint32_t total = w * h, step = gridDim.x * blockDim.x, first = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t n = first < total ? (total - 1u - first) / step + 1u : 0u;     // counted first, as in color_matrix_kernel
     uint32_t i = first;
@@ -236,15 +236,7 @@ __global__ void __launch_bounds__(256) apply_matte_kernel(uint8_t* __restrict__ 
         const uint32_t pa = v >> 24;
         if (pa == 0u) { *p = matte_bgra; continue; }
         if (pa == 255u) continue;
-        const float paf = __fmul_rn((float)(int)pa, a2f);
-        const float m_a = __fmul_rn(__fsub_rn(1.0f, paf), ma);
-        const float fa = __fadd_rn(m_a, paf);
-        auto ch = [&](uint32_t byte, float m) {
-            const float lin = __fdiv_rn(__fadd_rn(__fmul_rn(__ldg(tb.t_lin + byte), paf), __fmul_rn(m, m_a)), fa);
-            return lut_encode(tb.lut16k, lin);
-        };
-        const uint32_t nb = ch(v & 0xffu, mb), ng = ch((v >> 8) & 0xffu, mg), nr = ch((v >> 16) & 0xffu, mr);
-        *p = nb | (ng << 8) | (nr << 16) | (uchar_clamp_ff(__fmul_rn(255.0f, fa)) << 24);
+        *p = matte_blend(v, pa, ml, tb);
     }
 }
 
@@ -406,6 +398,7 @@ __global__ void __launch_bounds__(256) apply_byte_maps_bgra8_kernel(uint8_t* __r
 // ---------------------------------------------------------------- pixel formats at the graph's edges (RGB24, RGBA, Gray, GrayAlpha <-> BGRA); own file for tests/cpu_emu
 #include "ifb_pixel_convert_kernel.cuh"
 #include "ifb_ycbcr_kernel.cuh"
+#include "ifb_ycbcr_enc_kernel.cuh"
 
 // ---------------------------------------------------------------- colour profiles to sRGB (matrix-shaper ICC, gray ICC, gAMA+cHRM, CICP); own file for tests/cpu_emu
 #include "ifb_profile_kernel.cuh"

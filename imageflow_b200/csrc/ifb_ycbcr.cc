@@ -4,16 +4,11 @@
 #include "ifb_prepare.h"
 
 namespace ifb {
-namespace {
 
-// the byte span [first, last) of a plane of `rows` rows of `row_bytes` bytes, `stride` apart
-struct Span { uintptr_t a, b; };
 Span span_of(const uint8_t* p, uint32_t stride, uint32_t rows, uint64_t row_bytes) {
     const uintptr_t a = reinterpret_cast<uintptr_t>(p);
     return {a, a + (uint64_t)(rows - 1) * stride + row_bytes};
 }
-
-}  // namespace
 
 uint32_t ycbcr_chroma_w(int32_t sampling, uint32_t w) {
     if (sampling == IFB200_YCBCR_444) return w;

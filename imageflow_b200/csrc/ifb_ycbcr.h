@@ -35,6 +35,10 @@ uint32_t ycbcr_chroma_h(int32_t sampling, uint32_t h);
 // Row bands of an item: ceil(h / 2) at 4:2:0, else h.
 uint32_t ycbcr_bands(uint32_t sampling, uint32_t h);
 
+// The byte span [a, b) of a plane of `rows` (>= 1) rows of `row_bytes` bytes, `stride` apart; two planes overlap when their spans do.
+struct Span { uintptr_t a, b; };
+Span span_of(const uint8_t* p, uint32_t stride, uint32_t rows, uint64_t row_bytes);
+
 // Empty when d is a valid descriptor, else why it is not; *code, when given, = IFB200_ERR_INVALID_ARGUMENT (its only status).
 std::string ycbcr_check(const ifb200_ycbcr_desc& d, int* code = nullptr);
 

@@ -11,7 +11,7 @@ import numpy as np
 
 from ._lib import (CanvasDesc, ColorDesc, ColorStep, DetectContentDesc, OrientDesc, OrientedResampleDesc, PixelConvertDesc, ProfilePlan,
                    ProfiledResampleDesc, ResampleDesc,
-                   RoundCornersDesc, RowsOrientedResampleDesc, RowsResampleDesc, SourceProfileDesc, ToSrgbDesc, WatermarkDesc, YcbcrDesc, lib)
+                   RoundCornersDesc, RowsOrientedResampleDesc, RowsResampleDesc, SourceProfileDesc, ToSrgbDesc, WatermarkDesc, YcbcrDesc, BgraToYcbcrDesc, lib)
 
 
 class Filter(enum.IntEnum):
@@ -1178,6 +1178,30 @@ def _plane(x) -> "PixelRows":
     return p
 
 
+# ---------------------------------------------------------------- BGRA into a JPEG encoder's Y, Cb, Cr planes (Batch.bgra_to_ycbcr)
+@dataclass
+class BgraToYcbcr:
+    """One frame of Batch.bgra_to_ycbcr: the encoder colour stage of MozjpegEncoder::write_frame (codecs/mozjpeg.rs:93-157) --
+    apply_matte over matte_bgra when alpha is meaningful, then libjpeg-turbo's RGB -> YCbCr and chroma downsampling at `sampling`.
+    src: a BGRA BitmapWindow or 4-channel rows (4-byte aligned); y, cb, cr: uint8 (H, W) CUDA tensors or one-channel PixelRows at any
+    pitch, y the size of src and cb, cr ycbcr_chroma_shape(sampling, w, h).  alpha_meaningful None takes the BitmapWindow's flag (False
+    for plain rows).  matte_bgra: B, G, R, A bytes; white unless the encoder is given a matte."""
+    src: object
+    sampling: int
+    y: object
+    cb: object
+    cr: object
+    alpha_meaningful: Optional[bool] = None
+    matte_bgra: tuple = (255, 255, 255, 255)
+
+
+_BGRA_TO_YCBCR_DESC_DTYPE = np.dtype({"names": [n for n, _ in BgraToYcbcrDesc._fields_],
+                                      "formats": [np.uint64 if t is C.c_void_p else ((np.uint8, (4,)) if n == "matte_bgra" else np.dtype(t))
+                                                  for n, t in BgraToYcbcrDesc._fields_],
+                                      "offsets": [getattr(BgraToYcbcrDesc, n).offset for n, _ in BgraToYcbcrDesc._fields_],
+                                      "itemsize": C.sizeof(BgraToYcbcrDesc)})
+
+
 # ---------------------------------------------------------------- colour profiles to sRGB (Batch.transform_to_srgb)
 @dataclass(frozen=True)
 class SourceProfile:
@@ -1695,6 +1719,51 @@ class Batch:
                 dst.alpha_meaningful = src.alpha_meaningful if isinstance(src, BitmapWindow) else PixelRows.of(src).channels in (2, 4)
         self._keep.append(keep)
         return outs
+
+    def bgra_to_ycbcr(self, jobs, stream=None) -> list:
+        """A JPEG encoder's colour stage on DEVICE frames -- apply_matte, then libjpeg-turbo's RGB -> YCbCr and chroma downsampling,
+        byte for byte the planes its compressor forms from JCS_EXT_BGRA -- all jobs in one kernel launch (none when no job has pixels),
+        asynchronous on `stream`.  jobs: iterable of BgraToYcbcr records; the sampling is always given (the reference lets evalchroma
+        choose it per image).  The source is only read.  Returns [(y, cb, cr)] per job.  Nothing is changed when an argument is
+        rejected."""
+        jobs = list(jobs)
+        rows, keep = [], []
+        for j in jobs:
+            if not isinstance(j, BgraToYcbcr):
+                raise FlowError(ErrorKind.InvalidArgument, f"not a BgraToYcbcr record: {j!r}")
+            s, py, pb, pr = PixelRows.of(j.src), _plane(j.y), _plane(j.cb), _plane(j.cr)
+            if s.channels != 4:
+                raise FlowError(ErrorKind.InvalidArgument, f"bgra_to_ycbcr reads a BGRA frame, not {s.channels}-channel rows")
+            ch, cw = ycbcr_chroma_shape(j.sampling, s.w, s.h)
+            if (py.w, py.h) != (s.w, s.h):
+                raise FlowError(ErrorKind.InvalidArgument, f"a {s.w}x{s.h} frame has a {s.w}x{s.h} Y plane, not {py.w}x{py.h}")
+            if (pb.h, pb.w) != (ch, cw) or (pr.h, pr.w) != (ch, cw):
+                raise FlowError(ErrorKind.InvalidArgument, f"a {s.w}x{s.h} frame at sampling {j.sampling} has {cw}x{ch} chroma planes, "
+                                                           f"not {pb.w}x{pb.h} and {pr.w}x{pr.h}")
+            matte = tuple(int(v) for v in j.matte_bgra)
+            if len(matte) != 4 or any(not 0 <= v <= 255 for v in matte):
+                raise FlowError(ErrorKind.InvalidArgument, f"matte_bgra is four bytes B, G, R, A, not {j.matte_bgra!r}")
+            am = j.alpha_meaningful if j.alpha_meaningful is not None else (isinstance(j.src, BitmapWindow) and j.src.alpha_meaningful)
+            rows.append((j.sampling, s.ptr, s.stride, py.ptr, py.stride, pb.ptr, pb.stride, pr.ptr, pr.stride, s.w, s.h, int(bool(am)), matte))
+            keep.append((s._keep, py._keep, pb._keep, pr._keep))
+        a = np.array(rows, _BGRA_TO_YCBCR_DESC_DTYPE) if rows else np.zeros(0, _BGRA_TO_YCBCR_DESC_DTYPE)
+        arr = (BgraToYcbcrDesc * len(jobs)).from_buffer(a)
+        buf = C.create_string_buffer(512)
+        _check(lib().ifb200_batch_bgra_to_ycbcr(self._h, arr, len(jobs), self._stream(stream), buf, 512), buf)
+        self._keep.append(keep)
+        return [(j.y, j.cb, j.cr) for j in jobs]
+
+    def to_ycbcr(self, src, sampling: int, alpha_meaningful: Optional[bool] = None, matte_bgra=(255, 255, 255, 255), stream=None):
+        """One frame from BGRA -- an (H, W, 4) uint8 CUDA tensor or a BitmapWindow -- to three new contiguous uint8 CUDA tensors
+        (y, cb, cr) on the batch's device, the planes a GPU JPEG encoder takes (Batch.bgra_to_ycbcr's semantics)."""
+        import torch
+        s = PixelRows.of(src)
+        ch, cw = ycbcr_chroma_shape(sampling, s.w, s.h)
+        dev = f"cuda:{self.device}"
+        y = torch.empty((s.h, s.w), dtype=torch.uint8, device=dev)
+        cb, cr = (torch.empty((ch, cw), dtype=torch.uint8, device=dev) for _ in range(2))
+        self.bgra_to_ycbcr([BgraToYcbcr(src, sampling, y, cb, cr, alpha_meaningful, matte_bgra)], stream)
+        return y, cb, cr
 
     def to_bgra(self, rows, opaque: bool = False, stream=None) -> "BitmapWindow":
         """One call from decoder rows -- an (H, W, C) uint8 CUDA tensor, C in 1..4, or PixelRows -- to a new BGRA BitmapWindow on the

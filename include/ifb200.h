@@ -319,6 +319,36 @@ typedef struct ifb200_ycbcr_desc {
     uint32_t       w, h;
 } ifb200_ycbcr_desc;
 
+/* One JPEG frame's encoder colour stage, the way back: a BGRA frame into the Y, Cb and Cr planes a GPU JPEG encoder takes (nvJPEG's
+ * nvjpegEncodeYUV), byte for byte what libjpeg-turbo's compressor holds before its DCT when it is fed apply_matte(src) as JCS_EXT_BGRA
+ * with jpeg_set_defaults (no smoothing) and the given sampling -- the reference's MozjpegEncoder::write_frame (codecs/mozjpeg.rs).
+ *   Matte   when alpha_meaningful != 0, each pixel is first flattened over matte_bgra exactly as ifb200_batch_apply_matte does
+ *           (graphics/blend.rs, linear light); the source is never written.  Alpha is then ignored, as libjpeg ignores it.
+ *   Colour  jccolor.c rgb_ycc_convert, >> arithmetic, results always in 0..255:
+ *             Y  = (19595 R + 38470 G + 7471 B + 32768) >> 16
+ *             Cb = (-11059 R - 21709 G + 32768 B + (128 << 16) + 32767) >> 16
+ *             Cr = (32768 R - 27439 G - 5329 B + (128 << 16) + 32767) >> 16
+ *   Sampling (jcsample.c), on the full-resolution Cb and Cr:
+ *     444  a copy: the chroma planes are w x h.
+ *     422  chroma ceil(w/2) x h; column i = (c[2i] + c[2i+1] + bias) >> 1, bias 0 at even i, 1 at odd i (h2v1_downsample).
+ *     420  chroma ceil(w/2) x ceil(h/2); sample (i, j) = (the 2 x 2 box at (2i, 2j) summed + bias) >> 2, bias 1 at even i, 2 at
+ *          odd i (h2v2_downsample).
+ *   A ragged last column or row is replicated at full resolution before the box sums (expand_right_edge and the preprocessor's
+ *   bottom-edge expansion): an odd width's last 4:2:0 sample is (2 (a + b) + bias) >> 2 of the last column's two rows.
+ * Only the visible samples are written: Y is w x h, each chroma plane ceil(w / h_factor) x ceil(h / v_factor).  The caller chooses the
+ * sampling (the reference lets evalchroma pick it per image).  The source is 4-byte aligned BGRA; each plane may sit at any byte
+ * address with any pitch that holds a row.  4:4:0, 4:1:1, grayscale output and smoothing are not covered. */
+typedef struct ifb200_bgra_to_ycbcr_desc {
+    int32_t        sampling;                /* enum ifb200_ycbcr_sampling */
+    const uint8_t* src; uint32_t src_stride;   /* w x h BGRA: 4-byte aligned pointer and stride; only read */
+    uint8_t*       y;  uint32_t y_stride;   /* w x h luma */
+    uint8_t*       cb; uint32_t cb_stride;  /* chroma planes at the sampling's size; each plane has its own pitch */
+    uint8_t*       cr; uint32_t cr_stride;
+    uint32_t       w, h;
+    int32_t        alpha_meaningful;        /* != 0: flatten over matte_bgra first (as ifb200_batch_apply_matte) */
+    uint8_t        matte_bgra[4];           /* B, G, R, A; white (255, 255, 255, 255) unless the encoder is given one */
+} ifb200_bgra_to_ycbcr_desc;
+
 /* A decoder's colour profile (the reference's SourceProfile, codecs/source_profile.rs:7-41, CMYK excluded) and the transform of a
  * frame to sRGB under it: transform_to_srgb(to_bgra(src, format), profile) as codecs/moxcms_transform.rs runs it with
  * lut_transform_opts() (relative colorimetric), for the profiles whose transform is a matrix-shaper.  Kinds:
@@ -555,6 +585,13 @@ int  ifb200_batch_pixel_convert(ifb200_batch* b, const ifb200_pixel_convert_desc
  * unknown sampling, a misaligned destination, a destination that overlaps a plane of its job), so an error means nothing is written.
  * A job of zero area is skipped unchecked.  There is no host-buffer variant. */
 int  ifb200_batch_ycbcr_to_bgra(ifb200_batch* b, const ifb200_ycbcr_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
+/* JPEG encoder colour stages (ifb200_bgra_to_ycbcr_desc) of n DEVICE frames in ONE kernel launch, none when no job has pixels; each
+ * plane byte is written once and nothing outside the source window and the planes is read or written.  Asynchronous on
+ * `cuda_stream`.  No job may write what another job of the same call reads or writes (not checked).  Every descriptor is checked
+ * before anything is planned or enqueued ("bgra_to_ycbcr job i: <why>", IFB200_ERR_INVALID_ARGUMENT: a null source or plane, a stride
+ * smaller than its row, an unknown sampling, a misaligned source, a plane that overlaps the source or another plane of its job), so an
+ * error means nothing is written.  A job of zero area is skipped unchecked.  There is no host-buffer variant. */
+int  ifb200_batch_bgra_to_ycbcr(ifb200_batch* b, const ifb200_bgra_to_ycbcr_desc* d, size_t n, void* cuda_stream, char* err, size_t err_cap);
 /* Colour profiles to sRGB (ifb200_to_srgb_desc, ifb200_source_profile) on n DEVICE windows in ONE kernel launch, none when no job
  * writes a pixel (SRGB jobs in place, zero-area jobs); asynchronous on `cuda_stream`.  Each destination byte is written once and
  * nothing outside the two windows is read.  Every descriptor is checked and every profile planned before anything is enqueued, so an
